@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — constraint-rows/sec of the zkevm-specs hot path on B200.
+"""bench.py — constraint-rows/sec of the zkevm-specs hot path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload W] [--scaling S]
+                    [--dump-outputs DIR]
 
 Main line (the bench contract): workload `evm` = BASELINE cfg2's generator scaled to the metric's 2^20
 rows — per GPU 2^18 groups `PUSH32 b, PUSH32 a, {ADD,SUB,MUL,DIV,MOD}, POP` = 2^20 execution steps,
@@ -11,18 +12,18 @@ of the bytecode / rw tables on the device, then check every execution step.
   value    : rows/s with all inputs resident in HBM (CUDA events on the launching stream)
   e2e      : rows/s through the C-ABI with HOST (pinned) buffers: H2D of tables + steps, index build,
              check, D2H of the result vector, all inside the timed region
-  roofline : algorithmic bytes of the check phase / its device time vs MEASURED_PEAKS.json, next to the
-             honest denominators: stored bytes (what sits in HBM) and DRAM traffic (ncu capture of THIS
-             build, profiles/, matched by source hash — null when the sources changed since the capture)
+  roofline : algorithmic bytes of the check phase / its device time vs MEASURED_PEAKS.json (or the H100 SXM
+             data sheet's 3.35 TB/s when that file is absent), next to the honest denominator: stored bytes
+             (what sits in HBM)
   cpu_baseline : the CPU oracle (a C port of the reference algorithm; the reference itself is pure
-             Python and absent on this box) on a bounded sample of the same workload
+             Python and not part of this repository) on a bounded sample of the same workload
 Extra objects on the same line (`--no-extras` skips them; they are not inside the main timed region):
   typed          : the same check with data-independent column widths (packing.TYPE_WIDTHS)
   circuits       : BASELINE cfg3 (state 2^18 rows), cfg4's copy circuit (2^20 rows), the bytecode circuit
                    (2^19 rows) and the public-inputs circuit (64 txs, 2^18 calldata bytes: 2.9e5 rows) on
                    canonical 32-byte cells, each with its own roofline
   strong_scaling : ONE 2^20-step witness split over the N ranks (tables replicated, step shards with
-                   a halo step, one collective) — north_star's "2^20-row witness at 1/2/4/8 B200"
+                   a halo step, one collective) — the 2^20-row witness at 1/2/4/8 GPUs
   block_trace    : the realistic variant — ONE whole-block trace (4,096 transactions over 1,024 contracts: BeginTx ..
                    STOP, EndTx each, EndBlock last) checked with the first / last step flags
   assign         : witness assignment on the device (bytecode 2^19 / state 2^18 / copy 2^20 rows from their compact host
@@ -31,6 +32,9 @@ Extra objects on the same line (`--no-extras` skips them; they are not inside th
                    in total) row-sharded over the N ranks
 Multi-GPU (torchrun): rows are sharded, tables replicated, then ONE collective on the result vectors
 (zk_allreduce_results: NCCL all-gather + fold); main line scaling "weak" (own 2^20-step shard per rank).
+--dump-outputs DIR: after the timed steps, the result vectors of the last timed step (what zk_fetch_result
+hands a caller: per-constraint first failing row and failure count) as DIR/first_fail.npy and
+DIR/fail_count.npy (float64, exact), so that two builds can be compared on the same seeded witness.
 """
 import argparse
 import hashlib
@@ -106,24 +110,13 @@ def algorithmic_bytes(n_steps, n_rw, n_bytecode, n_constraints):
 
 
 def source_hash() -> str:
-    """hash of the CUDA sources: ties a profiles/ capture to the build it was taken from"""
+    """hash of the CUDA sources: ties a bench line to the build it was taken from"""
     h = hashlib.sha256()
     csrc = os.path.join(ROOT, "zkevm-specs_b200", "csrc")
     for f in sorted(os.listdir(csrc)):
         if f.endswith((".cu", ".cuh")):
             h.update(open(os.path.join(csrc, f), "rb").read())
     return h.hexdigest()[:16]
-
-
-def load_capture():
-    """profiles/current_capture.json: {"source_hash", "dram_bytes_per_check", "kernels": {...}} written by
-    tools/traffic_from_ncu.py from an `ncu --set full` capture of this command; used only when its
-    source_hash matches the sources on disk"""
-    try:
-        c = json.load(open(os.path.join(ROOT, "profiles", "current_capture.json")))
-        return c if c.get("source_hash") == source_hash() else None
-    except Exception:  # noqa: BLE001
-        return None
 
 
 def _cpu_port_worker(args):
@@ -164,7 +157,7 @@ def cpu_port(sample_groups: int, seed: int, threads: int):
 
 def run_reference_arm(args, rank, world):
     """--impl reference: the reference's algorithm on the host cores.  The reference is pure
-    Python and /root/reference is absent on the GPU box, so this times the C port (oracle/) with
+    Python and not part of this repository, so this times the C port (oracle/) with
     one process per core (rows are independent: that is how the reference would use the cores).
     A step = every core checks its own bounded sample of the cfg2 trace; the sample is sized from
     a calibration step so that the K timed steps end within ~2 minutes."""
@@ -230,8 +223,8 @@ class Harness:
             box = [self.ctx.nccl_unique_id() if rank == 0 else None]
             dist.broadcast_object_list(box, src=0)
             self.ctx.nccl_init(world, rank, box[0])
-        self.peak = 6650.0
-        self.peak_source = "fallback 6.65 TB/s"
+        self.peak = 3350.0
+        self.peak_source = "H100 SXM data sheet, 3.35 TB/s"
         try:
             self.peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
             self.peak_source = "MEASURED_PEAKS.json (burst copy)"
@@ -515,6 +508,8 @@ def main():
                          "columns stored once (packing.pack_matrix); typed (= packed): data-independent widths by "
                          "column type (packing.TYPE_WIDTHS); both through zk_upload_*_packed.  canonical: 32-byte "
                          "cells through zk_upload_*")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's result vectors as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -634,21 +629,21 @@ def main():
     clocks = sampler.stop()
     rows_per_step = n_total if strong else world * n_steps
     value = rows_per_step * args.steps / (ms / 1e3)
+    if args.dump_outputs and rank == 0:
+        ff, fc = ctx.fetch_result(native.CIRCUIT_EVM, stream)  # left on the device by the last timed step
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "first_fail.npy"), ff.astype(np.float64))
+        np.save(os.path.join(args.dump_outputs, "fail_count.npy"), fc.astype(np.float64))
 
     # ---- roofline of the check phase, device-timed per launch inside the library ----------------
     idx_ms, chk = h.phases(native.CIRCUIT_EVM, 0, n_steps, row_base, 0, min(args.steps, 50))
     bytes_alg = algorithmic_bytes(n_steps, n_rw, n_bc, n_constraints)
-    cap = load_capture() if (args.groups == (1 << 18) and args.storage == "adaptive" and not strong) else None
     roofline = roofline_of(h, chk, bytes_alg, stored=storage["stored_bytes"],
                            kernel="evm check phase: k_evm_classify + k_evm_scatter + k_evm_push_pos + k_evm_gadget<MUL|ADD|POP, POS>",
                            index_build_ms=idx_ms, achieved_stored_gbs=storage["stored_bytes"] / (chk / 1e3) / 1e9,
                            note="frac uses SURVEY.md 8(d)'s canonical bytes (every cell at 32 B); the kernels read the "
-                                "narrow stored columns, so stored_frac / dram_frac are the figures that bound them — they "
-                                "are latency- / issue-bound, not byte-bound (profiles/README.md)")
-    if cap:
-        roofline["traffic"] = cap["dram_bytes_per_check"]
-        roofline["dram_frac"] = cap["dram_bytes_per_check"] / (chk / 1e3) / 1e9 / h.peak
-        roofline["ncu"] = {k: cap[k] for k in ("capture", "kernels", "kernel_ms_sum") if k in cap}
+                                "narrow stored columns, so stored_frac is the figure that bounds them — they are "
+                                "latency- / issue-bound, not byte-bound (DESIGN.md)")
 
     # ---- e2e: host buffers through the C-ABI, copies inside the timed region --------------------
     # Every step ships its inputs from pinned host memory, builds the indexes, checks, and reads the result

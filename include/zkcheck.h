@@ -1,5 +1,5 @@
 /*
- * zkcheck.h — C-ABI of libzkcheck.so, the B200 constraint checker behind the
+ * zkcheck.h — C-ABI of libzkcheck.so, the H100 constraint checker behind the
  * zkevm-specs Python API.
  *
  * The reference (privacy-scaling-explorations/zkevm-specs @ 6058c68) has no FFI;

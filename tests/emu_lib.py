@@ -26,7 +26,7 @@ def lib():
             os.makedirs(os.path.dirname(OUT), exist_ok=True)
             # host-only build with plain g++: the gate programs are __host__ __device__ functions, the
             # kernels and other device-only declarations sit under #ifdef __CUDACC__ (20 s instead of the
-            # 5 minutes nvcc needs to also generate sm_100a code nobody runs here)
+            # 5 minutes nvcc needs to also generate sm_90a code nobody runs here)
             subprocess.run(["g++", "-x", "c++", "-std=c++17", "-O1", "-fPIC", "-shared", "-D__host__=", "-D__device__=",
                             "-D__forceinline__=inline", "-D__noinline__=__attribute__((noinline))", "-w",
                             "-o", OUT, SRC], check=True)

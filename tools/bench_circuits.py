@@ -1,12 +1,12 @@
 """Supplementary measurements (not the bench.py contract): BASELINE.json's cfg3 / cfg4 / cfg5 on one
-B200 — device time, rows/s and achieved GB/s (canonical algorithmic bytes, SURVEY.md §8d) of every
+H100 — device time, rows/s and achieved GB/s (canonical algorithmic bytes, SURVEY.md §8d) of every
 row circuit, each pass including its lookup-index work, for canonical and packed storage:
   state circuit  cfg3: 2^18 rows;  cfg5 share: 2^21 rows
   copy circuit   cfg4: 2^20 rows;  cfg5 share: 2^19 rows
   bytecode circuit     cfg5 share: 2^19 rows
   evm circuit          cfg5 share: 2^20 steps (bench.py's workload)
 and the cfg5 "super circuit" aggregate (sum of rows / sum of device time; each circuit is checked
-against its own tables, DESIGN.md section 7).  One JSON line per measurement; committed under profiles/."""
+against its own tables, DESIGN.md section 7).  One JSON line per measurement on stdout."""
 import json
 import os
 import sys

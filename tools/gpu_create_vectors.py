@@ -1,5 +1,5 @@
 """ErrorOutOfGasCREATE, ErrorOutOfGasSloadSstore and CREATE / CREATE2 vectors (tests/golden/evm26.npz, evm25.npz, evm24.npz) through the C-ABI on cuda:0 against the oracle, array for array.
-Small enough to run under compute-sanitizer (tools/gpu_r02_w.sh)."""
+Small enough to run under compute-sanitizer."""
 import os
 import sys
 

@@ -1,7 +1,7 @@
 // api.cu — the C-ABI of libzkcheck.so (include/zkcheck.h): context, uploads, lookup-index
 // cache, kernel dispatch, result transport.  Unity build: the circuit kernels are included
-// below so the whole library is one translation unit (nvcc -gencode arch=compute_100a,
-// code=sm_100a).  No torch types cross this boundary.
+// below so the whole library is one translation unit (nvcc -gencode arch=compute_90a,
+// code=sm_90a).  No torch types cross this boundary.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <stdio.h>
@@ -110,7 +110,7 @@ struct zk_ctx {
   ResultBuf res[ZK_N_CIRCUITS];
   std::string err;
   u64 launches = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   u32* resp_bitmap = nullptr;  // ResponsibleOpcode bitmap of the fixed table (8 KiB)
   u64 resp_bitmap_version = ~0ull;
   unsigned char* stage = nullptr;  // device staging (zk_upload_bytecode_table_from_code)

@@ -23,7 +23,7 @@ ZK_HD Fr wcell(const WitnessDev& w, u32 col, u64 row) {
   return ld_col(w.base + w.off[col], w.width[col], row);
 }
 // Storage layout a row-checker instance is compiled for.  L_CANON: every column holds canonical 32-byte
-// cells (zk_upload_columns) — a cell load is one address add + one LDG.256; L_ANY: per-column widths
+// cells (zk_upload_columns) — a cell load is one address add + two LDG.128; L_ANY: per-column widths
 // (packed uploads) through the generic branch-free loader, ~20 more instructions per load.  The host
 // picks the instance from the resident matrix's widths; results are identical.
 enum { L_ANY = 0, L_CANON = 1 };
@@ -49,10 +49,9 @@ ZK_HD u64 rot_back(const WitnessDev& w, u64 row, bool wrap) {
 }
 
 #ifdef __CUDACC__
-// (Two alternatives for the canonical row checkers were built and measured, then dropped — profiles/README.md,
-// r02: a 4-deep TMA tile pipeline with one 128-thread CTA per SM made the gate program itself the bound
-// (6 % warps active, issue slots 18 % busy, 0.35 of HBM vs 0.55 for direct loads); prefetch.global.L2 of
-// the thread's next row cost more issue slots than it hid latency (0.51 / 0.41 / 0.35 vs 0.55 / 0.51 / 0.43).)
+// (Two alternatives for the canonical row checkers were built and dropped: a 4-deep TMA tile pipeline with
+// one 128-thread CTA per SM made the gate program itself the bound (few warps active, low issue rate);
+// prefetch.global.L2 of the thread's next row cost more issue slots than it hid latency.)
 // Stage a small read-only table into shared memory with ONE bulk asynchronous copy
 // (cp.async.bulk, the 1-D TMA path: SASS UBLKCP) completing on an mbarrier.  Called by every
 // thread of the block; returns when the bytes are visible to all of them.  `bytes` must be a

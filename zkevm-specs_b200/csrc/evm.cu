@@ -453,7 +453,7 @@ ZK_HD u64 div128by64(u64 u1, u64 u0, u64 v) {
 // q = n / d for d != 0 (only MOD steps pay for it).  Knuth's algorithm D with 64-bit digits on
 // operands shifted so that the divisor's top bit is bit 255: always 4 quotient digits, static limb
 // indices, no data-dependent trip count — so the lanes of a warp stay together (the bit-serial
-// shift-subtract it replaces ran up to 256 iterations in the slowest lane: profiles/README.md v20).
+// shift-subtract it replaces ran up to 256 iterations in the slowest lane).
 ZK_HD void div256(const u64 n[4], const u64 d[4], u64 q[4]) {
   q[0] = q[1] = q[2] = q[3] = 0;
   if (cmp256(n, d) < 0) return;
@@ -2030,7 +2030,7 @@ __global__ void __launch_bounds__(1024) k_evm_scatter(EvmSort so, u32 n) {
 // one thread per step for the gadgets whose work is a handful of independent lookups.
 // POS = both tables positional (known to the host from the read-back flag): that instance is compiled
 // with pos_mode = 1, i.e. without any hash-index code — these kernels were stalling on instruction
-// fetch (profiles/README.md v20: "no instruction" 2-3 per issue), the executed path is now half as long.
+// fetch ("no instruction" stalls), the executed path is now half as long.
 // POS: 0 = hash indexes, 1 = both tables positional, 2 = positional AND narrow (StepCtx::narrow)
 template <int G, int POS>
 __device__ __forceinline__ void bucket_steps(const WitnessDev& w, const CheckRange& rg, const EvmTables& t,
@@ -2054,17 +2054,15 @@ __device__ __forceinline__ void bucket_steps(const WitnessDev& w, const CheckRan
     else gadget_pop(s, live);
   }
 }
-// minimum resident blocks per SM (= register caps of 168 / 128): measured sweep in
-// profiles/r01_v25_launch_bounds_sweep.json — (3, 4) cuts the check phase from 0.539 to 0.443 ms
+// minimum resident blocks per SM (= register caps of 168 / 128); override with -D to sweep them
 #ifndef ZK_GADGET_MINBLOCKS
 #define ZK_GADGET_MINBLOCKS 3
 #endif
 #ifndef ZK_PUSH_MINBLOCKS
 #define ZK_PUSH_MINBLOCKS 4
 #endif
-// ADD / SUB and POP are latency-bound on three dependent round trips (8-9 long-scoreboard stalls per issue,
-// profiles/r02_m_top_kernels_ncu_full.csv): 6 resident blocks (80 registers; POP without a spill, ADD with 216 bytes)
-// beat 3 (142 / 107 registers) by 3 % of the check phase (profiles/r02_m_launch_bound_variants.json)
+// ADD / SUB and POP are latency-bound on three dependent round trips (long-scoreboard stalls): 6 resident
+// blocks (80 registers) keep more steps in flight than 3 (142 / 107 registers) at the price of a few spills
 #ifndef ZK_ADD_MINBLOCKS
 #define ZK_ADD_MINBLOCKS 6
 #endif
@@ -2152,7 +2150,7 @@ __global__ void __launch_bounds__(128, ZK_PUSH_MINBLOCKS) k_evm_push_pos(const _
 // iteration): sub-lane L of a half owns pushed bytes L and L+16 of its step, so the warp-synchronous
 // hash probes of a step's 34 bytecode lookups run side by side.  Halving the lanes per step halves
 // the warp-instructions per step and doubles the steps in flight per warp; the kernel is
-// latency-bound on ~8 dependent memory round trips per step (profiles/README.md, v7).  All 32 lanes
+// latency-bound on ~8 dependent memory round trips per step.  All 32 lanes
 // call every warp-synchronous lookup together; a half without a step (odd count) or whose step
 // already failed passes live = false.
 __global__ void __launch_bounds__(128, 4) k_evm_push_hash(const __grid_constant__ WitnessDev w, const __grid_constant__ CheckRange rg, const __grid_constant__ EvmTables t, const __grid_constant__ ResultDev res,

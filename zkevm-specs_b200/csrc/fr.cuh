@@ -1,4 +1,4 @@
-// fr.cuh — BN254 scalar-field cells on the device (sm_100a).
+// fr.cuh — BN254 scalar-field cells on the device (sm_90a).
 //
 // Device-side counterpart of the reference's FQ (src/zkevm_specs/util/arithmetic.py:41-63,
 // arithmetic in py_ecc.bn128.FQ).  A cell is 4 little-endian uint64 limbs holding the
@@ -32,8 +32,9 @@ struct Fr {
 // 2^64 in Montgomery form (2^64 * 2^256 mod p)
 #define ZK_MONT_TWO64 Fr{{0xb4c6edf97c5fb586ull, 0x708c8d50bfeb93beull, 0x9ffd1de404f7e0efull, 0x215b02ac9a392866ull}}
 
-// One 256-bit load per cell: LDG.E.256 on sm_100a; a warp reading 32 consecutive rows of a
-// column moves 1 KiB in one instruction.  .nc: witness/table cells are read-only.
+// A 32-byte cell is two independent 128-bit loads (LDG.E.128, the widest global load sm_90a has),
+// issued back to back; a warp reading 32 consecutive rows of a column moves 1 KiB in two
+// instructions.  .nc: witness/table cells are read-only.
 // (The host branch exists only so that tests/emu can run the SAME gate programs on the CPU
 // for local debugging before a GPU call; the product never executes it.)
 #define ZK_HD __host__ __device__ __forceinline__
@@ -41,9 +42,11 @@ struct Fr {
 ZK_HD Fr ld_cell(const u64* p) {
   Fr r;
 #ifdef __CUDA_ARCH__
-  asm volatile("ld.global.nc.v4.u64 {%0,%1,%2,%3}, [%4];"
-               : "=l"(r.l[0]), "=l"(r.l[1]), "=l"(r.l[2]), "=l"(r.l[3])
-               : "l"(p));
+  asm volatile(
+      "ld.global.nc.v2.u64 {%0,%1}, [%4];\n\t"
+      "ld.global.nc.v2.u64 {%2,%3}, [%4+16];"
+      : "=l"(r.l[0]), "=l"(r.l[1]), "=l"(r.l[2]), "=l"(r.l[3])
+      : "l"(p));
 #else
   r.l[0] = p[0]; r.l[1] = p[1]; r.l[2] = p[2]; r.l[3] = p[3];
 #endif
@@ -57,7 +60,7 @@ ZK_HD Fr ld_cell(const u64* p) {
 // the bench: 3.4 GB -> 0.70 GB).  The branch is uniform: the width is a per-column constant.
 // Device form is BRANCH-FREE (three predicated loads, one executes): with branches the compiler
 // cannot batch a thread's independent cell loads ahead of the compares, and the gate programs are
-// latency-bound on exactly that (profiles/README.md v12).  Widths <= 8 load the aligned 8-byte
+// latency-bound on exactly that.  Widths <= 8 load the aligned 8-byte
 // word that contains the value (a w-byte integer at a multiple of w never straddles one; columns
 // start at multiples of 32 and are padded to 32) and shift/mask it out.
 ZK_HD Fr ld_col(const unsigned char* p, u32 width, u64 row) {
@@ -74,7 +77,8 @@ ZK_HD Fr ld_col(const unsigned char* p, u32 width, u64 row) {
       "setp.eq.u32 pc, %5, 32;\n\t"
       "@pa ld.global.nc.u64 %0, [%6];\n\t"
       "@pb ld.global.nc.v2.u64 {%0,%1}, [%4];\n\t"
-      "@pc ld.global.nc.v4.u64 {%0,%1,%2,%3}, [%4];\n\t"
+      "@pc ld.global.nc.v2.u64 {%0,%1}, [%4];\n\t"
+      "@pc ld.global.nc.v2.u64 {%2,%3}, [%4+16];\n\t"
       "}"
       : "+l"(r.l[0]), "+l"(r.l[1]), "+l"(r.l[2]), "+l"(r.l[3])
       : "l"(a), "r"(lw), "l"(a & ~7ull));

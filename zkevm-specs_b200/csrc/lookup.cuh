@@ -143,7 +143,7 @@ ZK_HD bool rows_identical(const TableDev& t, u32 a, u32 b) {
 // to look up pass active = false).  Lanes finish their bucket runs after different numbers of
 // slots; the loop runs until every lane of the mask is done (warp-uniform trip count), so the
 // warp leaves the loop CONVERGED.  With a plain data-dependent `break` each lane ran the rest
-// of its gate program alone (measured: 1-2 active threads per instruction, profiles/r01_v4).
+// of its gate program alone (1-2 active threads per instruction).
 template <int NK>
 ZK_HD int probe_slots(const IndexDev& ix, const u64* slots, u32 slot_mask, const Fr& h, const Fr (&key)[NK],
                       u32* row, unsigned mask, bool active, u32* slot_out = nullptr) {
@@ -216,8 +216,7 @@ ZK_HD bool pos_enabled(const IndexDev& ix) { return ix.pos_ok != nullptr && ld_u
 // The tail run (keys whose tail column holds tail_val: the rw table's Start padding rows, stored after the dense head)
 // is the same computation on another window of rows — base, limit and row offset switch, the loads and compares are
 // shared.  (Round 1 had the tail as an out-of-line function taking the key array by reference: that single call pinned
-// every caller's key array in local memory — 160-750 B of stack traffic per row in every kernel with a positional
-// lookup; profiles/README.md r02.)
+// every caller's key array in local memory — stack traffic per row in every kernel with a positional lookup.)
 template <int NK, bool NARROW = false>
 ZK_HD int pos_lookup_dense(const IndexDev& ix, const Fr (&key)[NK], u32* row, bool active, const u64* base0 = nullptr,
                            int extra_col = -1, Fr* extra = nullptr, int extra_col2 = -1, Fr* extra2 = nullptr) {
@@ -293,7 +292,9 @@ ZK_HD void ld_head_ent(const HeadEnt* e, u64* claim, u32* head, u32* len, u64 h[
 #ifdef __CUDA_ARCH__
   u64 hl;
   asm volatile("ld.global.nc.v2.u64 {%0,%1}, [%2];" : "=l"(*claim), "=l"(hl) : "l"(e));
-  asm volatile("ld.global.nc.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(h[0]), "=l"(h[1]), "=l"(h[2]), "=l"(h[3]) : "l"(e->h));
+  asm volatile("ld.global.nc.v2.u64 {%0,%1}, [%4];\n\t"
+               "ld.global.nc.v2.u64 {%2,%3}, [%4+16];"
+               : "=l"(h[0]), "=l"(h[1]), "=l"(h[2]), "=l"(h[3]) : "l"(e->h));
   *head = (u32)hl;
   *len = (u32)(hl >> 32);
 #else

@@ -26,7 +26,7 @@ FLAG_WRAP, FLAG_EVM_FIRST_STEP, FLAG_EVM_LAST_STEP = 1, 2, 4
 ERR_ASSERT, ERR_LOOKUP_UNSAT, ERR_LOOKUP_AMBIGUOUS, ERR_RANGE_RAISE, ERR_VALUE, ERR_NOT_IMPLEMENTED = range(6)
 PASS = 0xFFFFFFFF
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 
@@ -44,7 +44,7 @@ def is_stale() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/api.cu (unity build) for sm_100a into libzkcheck.so, in-tree."""
+    """Compile csrc/api.cu (unity build) for sm_90a into libzkcheck.so, in-tree."""
     if not force and not is_stale():
         return LIB_PATH
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
