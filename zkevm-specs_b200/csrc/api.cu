@@ -123,7 +123,7 @@ struct zk_ctx {
   // own stream next to the hot kernels; forked after the scatter, joined before the check returns to the caller's stream
   cudaStream_t evm_aux = nullptr;
   cudaEvent_t evm_fork_ev = nullptr, evm_join_ev = nullptr;
-  int evm_tx_overlap = -1;  // -1 = not read yet (env ZKCHECK_TX_OVERLAP, default 1)
+  int evm_tx_overlap = 1;  // env ZKCHECK_TX_OVERLAP at context creation ("0..." = in-line order)
   int evm_occ[20] = {0};  // resident blocks per SM of the gate-program kernels (0 = not queried yet)
   std::unordered_map<const void*, int> occ;  // same, row-circuit kernels (keyed by kernel)
   BlockStats* block_stats = nullptr;  // k_evm_block_stats output
@@ -179,6 +179,14 @@ extern "C" int zk_ctx_create(int device_ordinal, zk_ctx** out) {
   zk_ctx* c = new zk_ctx();
   c->device = device_ordinal;
   cudaDeviceGetAttribute(&c->sm_count, cudaDevAttrMultiProcessorCount, device_ordinal);
+  // test seam: ZKCHECK_SM_COUNT = an integer in [1, SMs] caps every grid as if the device had that many SMs, so that a
+  // trace of a few thousand steps makes every thread of a persistent grid walk several rows; anything else is ignored
+  if (const char* e_ = getenv("ZKCHECK_SM_COUNT")) {
+    char* end = nullptr;
+    const long v = strtol(e_, &end, 10);  // an overflow saturates to LONG_MAX / MIN, outside the range
+    if (end != e_ && *end == '\0' && v >= 1 && v <= c->sm_count) c->sm_count = (int)v;
+  }
+  if (const char* e_ = getenv("ZKCHECK_TX_OVERLAP")) c->evm_tx_overlap = e_[0] == '0' ? 0 : 1;
   // defaults: fixed 253-bit constants (callers normally draw their own after fixing the witness)
   c->chal[ZK_CHALLENGE_KECCAK] = Fr{{0x9b97f4a7c15f39ccull, 0x0d6e8feb86659fd9ull, 0x3c2b2ae3d27d4eb4ull, 0x1165667b19e3779full}};
   c->chal[ZK_CHALLENGE_LOOKUP] = Fr{{0x2545f4914f6cdd1dull, 0x5851f42d4c957f2dull, 0x14057b7ef767814full, 0x0fe3a95bd3a1c8e7ull}};
@@ -1340,10 +1348,6 @@ static int check_evm(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStrea
   // persistent grids fill the device, and its long per-thread chains run underneath them
   bool tx_forked = false;
   if (group_n[KG_TX]) {
-    if (ctx->evm_tx_overlap < 0) {
-      const char* e_ = getenv("ZKCHECK_TX_OVERLAP");
-      ctx->evm_tx_overlap = (e_ && e_[0] == '0') ? 0 : 1;
-    }
     if (ctx->evm_tx_overlap) {
       if (!ctx->evm_aux) {
         CK(ctx, cudaStreamCreateWithFlags(&ctx->evm_aux, cudaStreamNonBlocking));
