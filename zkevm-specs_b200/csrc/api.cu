@@ -85,7 +85,9 @@ struct Index {
   u64* slots = nullptr;
   size_t cap = 0;
   u32 pos_kind = ZK_POS_NONE;
-  u32* pos_flag = nullptr;  // device flag written by k_pos_verify
+  u32* pos_flag = nullptr;  // device flag written by k_index_prepare
+  u32* pos_part = nullptr;  // its per-block flag pairs
+  u64 pos_part_cap = 0;     // blocks
   HeadEnt* heads = nullptr;  // ZK_POS_RUNS heads index
   u32* heads_aux = nullptr;  // [ZK_HEADS_CAP] head list, [1] count
   u64 built_version = ~0ull;
@@ -115,9 +117,10 @@ struct zk_ctx {
   u64 resp_bitmap_version = ~0ull;
   unsigned char* stage = nullptr;  // device staging (zk_upload_bytecode_table_from_code)
   size_t stage_cap = 0;
-  unsigned char* evm_sort = nullptr;  // EvmSort arrays: bucket[cap] | sorted[cap] | hist, cursor, offs
+  unsigned char* evm_sort = nullptr;  // EvmSort arrays: bucket[cap] | sorted[cap] | hist, cursor, done, offs
   size_t evm_sort_cap = 0;
-  u32* evm_hist_host = nullptr;  // pinned: histogram + positional flag read back after k_evm_classify
+  u32* evm_hist_host = nullptr;  // pinned, mapped: histogram + positional flag, written by k_evm_classify's last block
+  u32* evm_hist_mapped = nullptr;  // its device address
   cudaEvent_t evm_hist_ev = nullptr;
   // the transaction-level group (k_evm_group<TX>: a few thousand threads, each a chain of dependent lookups) runs on its
   // own stream next to the hot kernels; forked after the scatter, joined before the check returns to the caller's stream
@@ -125,6 +128,7 @@ struct zk_ctx {
   cudaEvent_t evm_fork_ev = nullptr, evm_join_ev = nullptr;
   int evm_tx_overlap = 1;  // env ZKCHECK_TX_OVERLAP at context creation ("0..." = in-line order)
   int evm_occ[20] = {0};  // resident blocks per SM of the gate-program kernels (0 = not queried yet)
+  int prep_occ = 0;       // blocks per SM of k_index_prepare's cooperative grid (0 = not queried yet)
   std::unordered_map<const void*, int> occ;  // same, row-circuit kernels (keyed by kernel)
   BlockStats* block_stats = nullptr;  // k_evm_block_stats output
   void* state_fold = nullptr;  // k_state_fold output: 64 bytes per resident state row
@@ -208,6 +212,7 @@ extern "C" void zk_ctx_destroy(zk_ctx* ctx) {
   for (auto* ix : ctx->indexes) {
     if (ix->slots) cudaFree(ix->slots);
     if (ix->pos_flag) cudaFree(ix->pos_flag);
+    if (ix->pos_part) cudaFree(ix->pos_part);
     if (ix->heads) cudaFree(ix->heads);
     if (ix->heads_aux) cudaFree(ix->heads_aux);
     delete ix;
@@ -956,37 +961,37 @@ static int ensure_index(zk_ctx* ctx, int table_id, const u32* key_cols, u32 n_ke
   d.heads_mask = ZK_HEADS_CAP - 1;
   d.heads_list = ix->heads_aux;
   d.heads_count = ix->heads_aux ? ix->heads_aux + ZK_HEADS_CAP : nullptr;
-  const unsigned grid = (unsigned)std::min<u64>((t.n_rows + 255) / 256, (u64)ctx->sm_count * 32);
-  if (t.n_rows && ix->pos_kind != ZK_POS_NONE) {
-    // verify the regular structure in one streaming pass; the flag stays 1 iff it holds
-    k_set_u32<<<1, 1, 0, st>>>(ix->pos_flag, 1u);
-    k_set_u32<<<1, 1, 0, st>>>(ix->pos_flag + 1, (u32)t.n_rows);
-    if (ix->heads) {
-      CK(ctx, cudaMemsetAsync(ix->heads, 0xFF, ZK_HEADS_CAP * sizeof(HeadEnt), st));
-      CK(ctx, cudaMemsetAsync(ix->heads_aux, 0, (ZK_HEADS_CAP + 1) * sizeof(u32), st));
-    }
-    if (ix->pos_kind == ZK_POS_RUNS && m.src_offsets) {
-      // unrolled by the library: regular by construction, heads + lengths straight from the offsets
-      k_heads_from_offsets<<<(unsigned)std::min<u64>((m.src_contracts + 255) / 256, 64), 256, 0, st>>>(
-          d, ix->pos_flag, m.src_offsets, m.src_contracts);
-      ctx->launches += 2;
-    } else {
-      k_pos_verify<<<grid, 256, 0, st>>>(d, ix->pos_flag);
-      ctx->launches += 2;
-      if (ix->pos_kind == ZK_POS_RUNS) {  // run lengths from the listed heads (a few thousand threads at most)
-        k_pos_runlen<<<16, 256, 0, st>>>(d);
-        ctx->launches += 1;
-      }
-    }
-    d.pos_ok = ix->pos_flag;
-  }
   if (t.n_rows) {
-    // generic hash index: cleared and built only if the table is not positional (both kernels
-    // return at once when the flag is set)
-    k_slots_clear<<<(unsigned)std::min<u64>((cap + 255) / 256, (u64)ctx->sm_count * 32), 256, 0, st>>>(ix->slots, cap, d.pos_ok);
-    k_index_build<<<grid, 256, 0, st>>>(d);
-    ctx->launches += 2;
-    CK(ctx, cudaGetLastError());
+    // verify pass, positional flag and (only if the table is not positional) the hash index: one cooperative launch
+    // (lookup.cuh k_index_prepare).  Its grid stays within the blocks the device keeps resident, and a small table
+    // gets a small grid.
+    if (!ctx->prep_occ) {
+      int occ = 0;
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_index_prepare, 256, 0) != cudaSuccess || occ < 1) occ = 1;
+      ctx->prep_occ = occ;
+    }
+    const u64 max_grid = (u64)ctx->prep_occ * ctx->sm_count;
+    const u64 work = std::max<u64>(t.n_rows, ix->pos_kind == ZK_POS_RUNS ? (u64)ZK_HEADS_CAP : 0);  // + clearing the heads
+    const unsigned grid = (unsigned)std::max<u64>(1, std::min<u64>((work + 1023) / 1024, max_grid));
+    IndexPrep prep{nullptr, nullptr, nullptr, 0};
+    if (ix->pos_kind != ZK_POS_NONE) {
+      if (!ix->pos_part || ix->pos_part_cap < grid) {
+        if (ix->pos_part) cudaFree(ix->pos_part);
+        ix->pos_part = nullptr;
+        CK(ctx, cudaMalloc(&ix->pos_part, 2 * (size_t)max_grid * sizeof(u32)));
+        ix->pos_part_cap = max_grid;
+      }
+      prep.ok = ix->pos_flag;
+      prep.part = ix->pos_part;
+      if (ix->pos_kind == ZK_POS_RUNS && m.src_offsets) {  // unrolled by the library: heads + lengths from the offsets
+        prep.offsets = m.src_offsets;
+        prep.n_contracts = m.src_contracts;
+      }
+      d.pos_ok = ix->pos_flag;
+    }
+    void* args[] = {(void*)&d, (void*)&prep};
+    CK(ctx, cudaLaunchCooperativeKernel((const void*)k_index_prepare, dim3(grid), dim3(256), args, 0, st));
+    ctx->launches += 1;
   } else if (!ix->empty_ready) {  // an empty table: clear the (minimum-size) slot array once
     CK(ctx, cudaMemsetAsync(ix->slots, 0xFF, cap * sizeof(u64), st));
   }
@@ -1250,11 +1255,12 @@ static int check_evm(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStrea
   if (n > ctx->evm_sort_cap) {
     if (ctx->evm_sort) cudaFree(ctx->evm_sort);
     ctx->evm_sort = nullptr;
-    CK(ctx, cudaMalloc(&ctx->evm_sort, up256(n) + up256(n * 4) + (3 * ZK_EVM_NB + 2) * sizeof(u32)));
+    CK(ctx, cudaMalloc(&ctx->evm_sort, up256(n) + up256(n * 4) + (3 * ZK_EVM_NB + 3) * sizeof(u32)));
     ctx->evm_sort_cap = n;
   }
   if (!ctx->evm_hist_host) {
-    CK(ctx, cudaHostAlloc(&ctx->evm_hist_host, (ZK_EVM_NB + 1) * sizeof(u32), cudaHostAllocDefault));
+    CK(ctx, cudaHostAlloc(&ctx->evm_hist_host, (ZK_EVM_NB + 1) * sizeof(u32), cudaHostAllocMapped));
+    CK(ctx, cudaHostGetDevicePointer((void**)&ctx->evm_hist_mapped, ctx->evm_hist_host, 0));
     CK(ctx, cudaEventCreateWithFlags(&ctx->evm_hist_ev, cudaEventDisableTiming));
   }
   EvmSort so;
@@ -1262,8 +1268,10 @@ static int check_evm(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStrea
   so.sorted = (u32*)(ctx->evm_sort + up256(ctx->evm_sort_cap));
   so.hist = (u32*)(ctx->evm_sort + up256(ctx->evm_sort_cap) + up256(ctx->evm_sort_cap * 4));
   so.cursor = so.hist + ZK_EVM_NB + 1;
-  so.offs = so.cursor + ZK_EVM_NB;
-  CK(ctx, cudaMemsetAsync(so.hist, 0, (2 * ZK_EVM_NB + 1) * sizeof(u32), st));
+  so.done = so.cursor + ZK_EVM_NB;
+  so.offs = so.done + 1;
+  so.host_hist = ctx->evm_hist_mapped;
+  CK(ctx, cudaMemsetAsync(so.hist, 0, (2 * ZK_EVM_NB + 2) * sizeof(u32), st));
   const WitnessDev wd = witness_dev(m);
   const unsigned sort_grid = (unsigned)((n + 1023) / 1024);
   // the narrow instance needs 40 registers: blocks of ZK_CLASSIFY_THREADS = 512 keep 48 warps resident per SM instead of 32
@@ -1276,8 +1284,7 @@ static int check_evm(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStrea
     cudaError_t e_ = cudaGetLastError();
     if (e_ != cudaSuccess) return fail_msg(ctx, std::string("launch of k_evm_classify: ") + cudaGetErrorString(e_));
   }
-  CK(ctx, cudaMemcpyAsync(ctx->evm_hist_host, so.hist, (ZK_EVM_NB + 1) * sizeof(u32), cudaMemcpyDeviceToHost, st));
-  CK(ctx, cudaEventRecord(ctx->evm_hist_ev, st));
+  CK(ctx, cudaEventRecord(ctx->evm_hist_ev, st));  // the histogram is in host memory once k_evm_classify is complete
   k_evm_scatter<<<sort_grid, 1024, 0, st>>>(so, (u32)n);
   ctx->launches += 2;
   {

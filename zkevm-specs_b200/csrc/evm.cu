@@ -1893,8 +1893,10 @@ struct EvmSort {
   unsigned char* bucket;  // [n] bucket of local step k (ZK_BK_NONE: it failed in the prologue)
   u32* hist;              // [ZK_EVM_NB + 1] steps per bucket; entry ZK_EVM_NB: 1 iff rw + bytecode tables are positional
   u32* cursor;            // [ZK_EVM_NB] scatter cursors (zeroed by the host)
+  u32* done;              // [1] k_evm_classify blocks finished (zeroed by the host)
   u32* offs;              // [ZK_EVM_NB + 1] first entry of each bucket in `sorted`
   u32* sorted;            // [n] local step indices, bucket by bucket
+  u32* host_hist;         // [ZK_EVM_NB + 1] mapped pinned host memory: `hist` as k_evm_classify's last block leaves it
 };
 
 // Table-derived constants of EndBlock (end_block.py:68-105).  The reference's tables are Python sets, so a
@@ -1987,6 +1989,20 @@ __global__ void __launch_bounds__(1024) k_evm_classify(const __grid_constant__ W
   __syncthreads();
   if (threadIdx.x < ZK_EVM_NB && s_hist[threadIdx.x]) atomicAdd(&so.hist[threadIdx.x], s_hist[threadIdx.x]);
   if (blockIdx.x == 0 && threadIdx.x == 0) so.hist[ZK_EVM_NB] = pos ? 1u : 0u;
+  // the last block to finish writes the whole histogram straight into the host's pinned buffer: the host reads it once
+  // this kernel is complete, and k_evm_scatter starts without waiting for a device-to-host copy
+  // (one fence per block, by the thread that counts the block: the barrier orders the block's histogram atomics before it)
+  __shared__ bool s_last;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    s_last = atomicAdd(so.done, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (s_last) {
+    __threadfence();
+    if (threadIdx.x <= ZK_EVM_NB) so.host_hist[threadIdx.x] = __ldcg(&so.hist[threadIdx.x]);
+  }
 }
 
 __global__ void __launch_bounds__(1024) k_evm_scatter(EvmSort so, u32 n) {

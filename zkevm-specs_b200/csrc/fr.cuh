@@ -126,7 +126,7 @@ ZK_HD Fr ld_col_narrow(const unsigned char* p, u32 width, u64 row) {
   return r;
 }
 // ld_col with the width known at compile time: one plain typed load (kernels that are
-// specialised for a storage layout, e.g. k_pos_verify over the type-width bytecode table)
+// specialised for a storage layout, e.g. the verify pass over the type-width bytecode table)
 template <int W>
 ZK_HD Fr ld_col_c(const unsigned char* p, u64 row) {
   Fr r;

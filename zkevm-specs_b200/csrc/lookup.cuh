@@ -14,6 +14,9 @@
 // table being a set).
 #pragma once
 #include "fr.cuh"
+#ifdef __CUDACC__
+#include <cooperative_groups.h>
+#endif
 
 namespace zk {
 
@@ -363,26 +366,37 @@ ZK_HD void pos_fail(u32* ok) {
 #endif
 }
 // ok[0] = flag, ok[1] = split row (initialised to n_rows).  Every row is checked against its predecessor:
-// inside a run the counter grows by one; the one allowed change of run is head -> tail.
-ZK_HD void pos_verify_dense_row(const IndexDev& ix, u32* ok, u64 row) {
-  const TableDev& t = ix.tab;
-  const Fr c = table_cell(t, ix.key_cols[0], row);
-  const bool tail = ix.tail_key >= 0 && fr_eq_u64(table_cell(t, ix.tail_col, row), ix.tail_val);
-  bool good = fr_fits64(c);
+// inside a run the counter grows by one; the one allowed change of run is head -> tail.  A counter cell is passed
+// as (fits 64 bits, limb 0); (pfit, p0, ptail) describe row - 1 and are ignored for row 0.
+ZK_HD void pos_verify_dense_step(u32* ok, u64 row, bool cfit, u64 c0, bool tail, bool pfit, u64 p0, bool ptail) {
+  bool good = cfit;
   if (row == 0) {
     if (tail) atomic_min_u32(ok + 1, 0u);
   } else {
-    const Fr p = table_cell(t, ix.key_cols[0], row - 1);
-    const bool ptail = ix.tail_key >= 0 && fr_eq_u64(table_cell(t, ix.tail_col, row - 1), ix.tail_val);
-    if (tail == ptail) good = good && fr_fits64(p) && p.l[0] != ~0ull && c.l[0] == p.l[0] + 1;
+    if (tail == ptail) good = good && pfit && p0 != ~0ull && c0 == p0 + 1;
     else if (tail) atomic_min_u32(ok + 1, (u32)row);
     else good = false;  // a head row after the tail
   }
   if (!good) pos_fail(ok);
 }
+ZK_HD bool pos_dense_tail(const IndexDev& ix, u64 row) {
+  return ix.tail_key >= 0 && fr_eq_u64(table_cell(ix.tab, ix.tail_col, row), ix.tail_val);
+}
+ZK_HD void pos_verify_dense_row(const IndexDev& ix, u32* ok, u64 row) {
+  const TableDev& t = ix.tab;
+  const Fr c = table_cell(t, ix.key_cols[0], row);
+  const bool tail = pos_dense_tail(ix, row);
+  Fr p = c;
+  bool ptail = tail;
+  if (row > 0) {
+    p = table_cell(t, ix.key_cols[0], row - 1);
+    ptail = pos_dense_tail(ix, row - 1);
+  }
+  pos_verify_dense_step(ok, row, fr_fits64(c), c.l[0], tail, fr_fits64(p), p.l[0], ptail);
+}
 // Claim an entry of the heads index for the run that starts at `row` with code hash (hlo, hhi).
 // `len` != nullptr: the run length is known (table unrolled by the library) and is stored at once;
-// otherwise the head is listed for k_pos_runlen, and listing more heads than half the index clears the
+// otherwise the head is listed for the run-length pass (pos_runlen_entry), and listing more heads than half the index clears the
 // flag (the caller of the known-length form checks the run count before).  A duplicate hash, a hash
 // cell beyond 128 bits or a full index clears the flag.
 ZK_HD void heads_insert(const IndexDev& ix, u32* ok, u64 row, const Fr& hlo, const Fr& hhi, const u32* len) {
@@ -527,44 +541,13 @@ ZK_HD int lookup(const IndexDev& ix, const Fr (&key)[NK], u32* row) {
 }
 
 #ifdef __CUDACC__
-// the generic hash index is only needed when the table is NOT positional
-__global__ void __launch_bounds__(256) k_index_build(IndexDev ix) {
-  if (pos_enabled(ix)) return;
-  const u64 stride = (u64)gridDim.x * blockDim.x;
-  for (u64 row = (u64)blockIdx.x * blockDim.x + threadIdx.x; row < ix.tab.n_rows; row += stride) index_insert_row(ix, row);
-}
-__global__ void __launch_bounds__(256) k_slots_clear(u64* slots, u64 n, const u32* skip_if_set) {
-  if (skip_if_set && *skip_if_set) return;
-  const u64 stride = (u64)gridDim.x * blockDim.x;
-  for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) slots[i] = ZK_EMPTY_SLOT;
-}
-__global__ void k_set_u32(u32* p, u32 v) { *p = v; }
-__global__ void __launch_bounds__(256) k_pos_runlen(IndexDev ix) {
-  if (ix.tab.n_rows == 0) return;
-  const u32 count = min(*ix.heads_count, ix.heads_mask + 1);
-  for (u32 k = blockIdx.x * blockDim.x + threadIdx.x; k <= count; k += gridDim.x * blockDim.x) pos_runlen_entry(ix, k, count);
-}
 // A bytecode table unrolled by the library itself (zk_upload_bytecode_table_from_code) is regular
 // by construction: its heads index is filled straight from the contract offsets — one thread per
 // CONTRACT instead of a pass over every table row — and only duplicate code hashes (or more
-// contracts than half the heads index, ZK_HEADS_CAP) still clear the flag.
-__global__ void __launch_bounds__(256) k_heads_from_offsets(IndexDev ix, u32* ok, const u64* offsets, u64 n_contracts) {
-  if (n_contracts > ((u64)ix.heads_mask + 1) / 2) {
-    if (blockIdx.x == 0 && threadIdx.x == 0) pos_fail(ok);
-    return;
-  }
-  for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < n_contracts; k += (u64)gridDim.x * blockDim.x) {
-    const u64 start = offsets[k], row = start + k;
-    const u32 len = (u32)(offsets[k + 1] - start);
-    heads_insert(ix, ok, row, table_cell(ix.tab, 0, row), table_cell(ix.tab, 1, row), &len);
-  }
-}
-__global__ void __launch_bounds__(256) k_pos_verify(IndexDev ix, u32* ok) {
+// contracts than half the heads index, ZK_HEADS_CAP) still clear the flag (k_index_prepare).
+// verify pass of a ZK_POS_RUNS table over its rows; `ok` is the calling block's flag
+__device__ void pos_verify_runs_rows(const IndexDev& ix, u32* ok) {
   const u64 stride = (u64)gridDim.x * blockDim.x;
-  if (ix.pos_kind == ZK_POS_DENSE) {
-    for (u64 row = (u64)blockIdx.x * blockDim.x + threadIdx.x; row < ix.tab.n_rows; row += stride) pos_verify_dense_row(ix, ok, row);
-    return;
-  }
   // the two layouts a bytecode table normally arrives in get plain typed loads; anything else goes
   // through the generic per-column-width loader
   const unsigned char* wd = ix.tab.width;
@@ -578,6 +561,135 @@ __global__ void __launch_bounds__(256) k_pos_verify(IndexDev ix, u32* ok) {
   } else {
     for (u64 row = row0; row < n; row += stride) pos_verify_run_row(ix, ok, row);
   }
+}
+// verify pass of a ZK_POS_DENSE table.  A warp takes tiles of 4 x 32 consecutive rows: every row's two cells (counter,
+// tail column) are loaded once, all eight loads of a lane in flight together, and the predecessor's cells come from
+// the neighbouring lane (lane 0: from lane 31 of the previous 32 rows, or one extra load at the tile's start).
+__device__ void pos_verify_dense_rows(const IndexDev& ix, u32* ok) {
+  constexpr int R = 4;
+  const TableDev& t = ix.tab;
+  const u64 n = t.n_rows;
+  const unsigned lane = threadIdx.x & 31;
+  const u64 warp = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((u64)gridDim.x * blockDim.x) >> 5;
+  const u32 col = ix.key_cols[0];
+  for (u64 tile = warp * (32 * R); tile < n; tile += n_warps * (32 * R)) {  // warp-uniform trip count
+    Fr c[R];
+    bool tl[R];
+#pragma unroll
+    for (int j = 0; j < R; j++) {
+      const u64 row = min(tile + 32 * j + lane, n - 1);
+      c[j] = table_cell(t, col, row);
+      tl[j] = pos_dense_tail(ix, row);
+    }
+    const u64 before = tile ? tile - 1 : 0;
+    const Fr pc = table_cell(t, col, before);
+    const bool pt = pos_dense_tail(ix, before);
+    bool pfit = fr_fits64(pc), ptail = pt;
+    u64 p0 = pc.l[0];
+#pragma unroll
+    for (int j = 0; j < R; j++) {
+      const bool cfit = fr_fits64(c[j]);
+      const u64 up0 = __shfl_up_sync(0xFFFFFFFFu, c[j].l[0], 1);
+      const bool upfit = __shfl_up_sync(0xFFFFFFFFu, (u32)cfit, 1) != 0;
+      const bool uptail = __shfl_up_sync(0xFFFFFFFFu, (u32)tl[j], 1) != 0;
+      const u64 last0 = __shfl_sync(0xFFFFFFFFu, c[j].l[0], 31);
+      const bool lastfit = __shfl_sync(0xFFFFFFFFu, (u32)cfit, 31) != 0;
+      const bool lasttail = __shfl_sync(0xFFFFFFFFu, (u32)tl[j], 31) != 0;
+      if (lane) {
+        p0 = up0;
+        pfit = upfit;
+        ptail = uptail;
+      }
+      const u64 row = tile + 32 * j + lane;
+      if (row < n) pos_verify_dense_step(ok, row, cfit, c[j].l[0], tl[j], pfit, p0, ptail);
+      p0 = last0;  // lane 0's predecessor in the next 32 rows
+      pfit = lastfit;
+      ptail = lasttail;
+    }
+  }
+}
+
+// Every part of an index build in ONE cooperative launch (grid-wide barriers between the phases):
+//   1. ZK_POS_RUNS: clear the heads index;
+//   2. the verify pass (or, for a bytecode table unrolled by the library, the heads straight from the contract
+//      offsets); each block verifies into its own flag pair and stores it in `part`;
+//   3. every block combines the blocks' flags; block 0 publishes them in `ok` (read by every later kernel);
+//      ZK_POS_RUNS tables that passed get their run lengths (pos_runlen_entry, one thread per listed head);
+//   4. only if the table is not positional (or has no positional kind): clear the slot array, then insert every row.
+// A positional table therefore costs one launch and no hash-index work, and no flag needs a reset beforehand: the
+// block flags are rewritten in full by every launch.
+struct IndexPrep {
+  u32* ok;             // [0] flag, [1] split row (ZK_POS_DENSE); nullptr when pos_kind == ZK_POS_NONE
+  u32* part;           // [2 * gridDim.x] per-block flag pairs
+  const u64* offsets;  // != nullptr: the bytecode table was unrolled by the library from these contract offsets
+  u64 n_contracts;
+};
+__global__ void __launch_bounds__(256) k_index_prepare(const __grid_constant__ IndexDev ix, const __grid_constant__ IndexPrep p) {
+  namespace cg = cooperative_groups;
+  cg::grid_group grid = cg::this_grid();
+  const u64 tid = (u64)blockIdx.x * blockDim.x + threadIdx.x, stride = (u64)gridDim.x * blockDim.x;
+  const u64 n = ix.tab.n_rows;
+  __shared__ u32 s_ok[2];
+  bool pos = false;
+  if (ix.pos_kind != ZK_POS_NONE) {
+    if (ix.pos_kind == ZK_POS_RUNS) {
+      const uint4 ones = make_uint4(~0u, ~0u, ~0u, ~0u);
+      uint4* h = (uint4*)ix.heads;
+      for (u64 i = tid; i < (u64)(ix.heads_mask + 1) * (sizeof(HeadEnt) / 16); i += stride) h[i] = ones;
+      for (u64 i = tid; i <= (u64)ix.heads_mask + 1; i += stride) ix.heads_list[i] = 0;  // list + count
+      grid.sync();
+    }
+    if (threadIdx.x == 0) {
+      s_ok[0] = 1;
+      s_ok[1] = (u32)n;
+    }
+    __syncthreads();
+    if (ix.pos_kind == ZK_POS_DENSE) {
+      pos_verify_dense_rows(ix, s_ok);
+    } else if (p.offsets) {
+      // regular by construction: only duplicate code hashes (or more contracts than half the heads index) clear the flag
+      if (p.n_contracts > ((u64)ix.heads_mask + 1) / 2) {
+        if (threadIdx.x == 0) s_ok[0] = 0;
+      } else {
+        for (u64 k = tid; k < p.n_contracts; k += stride) {
+          const u64 start = p.offsets[k], row = start + k;
+          const u32 len = (u32)(p.offsets[k + 1] - start);
+          heads_insert(ix, s_ok, row, table_cell(ix.tab, 0, row), table_cell(ix.tab, 1, row), &len);
+        }
+      }
+    } else {
+      pos_verify_runs_rows(ix, s_ok);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      p.part[2 * blockIdx.x] = s_ok[0];
+      p.part[2 * blockIdx.x + 1] = s_ok[1];
+    }
+    grid.sync();
+    u32 good = 1, split = (u32)n;
+    for (u32 b = threadIdx.x; b < gridDim.x; b += blockDim.x) {
+      good &= __ldcg(&p.part[2 * b]);
+      split = min(split, __ldcg(&p.part[2 * b + 1]));
+    }
+    pos = __syncthreads_and((int)good) != 0;
+    if (threadIdx.x == 0) s_ok[1] = (u32)n;
+    __syncthreads();
+    if (split < (u32)n) atomicMin(&s_ok[1], split);
+    __syncthreads();
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+      p.ok[0] = pos ? 1u : 0u;
+      p.ok[1] = s_ok[1];
+    }
+    if (pos && ix.pos_kind == ZK_POS_RUNS && !p.offsets) {  // run lengths from the listed heads
+      const u32 count = min(__ldcg(ix.heads_count), ix.heads_mask + 1);
+      for (u64 k = tid; k <= count; k += stride) pos_runlen_entry(ix, (u32)k, count);
+    }
+  }
+  if (pos) return;  // uniform over the grid
+  const ulonglong2 empty = make_ulonglong2(ZK_EMPTY_SLOT, ZK_EMPTY_SLOT);
+  for (u64 i = tid; i < ((u64)ix.mask + 1) / 2; i += stride) ((ulonglong2*)ix.slots)[i] = empty;
+  grid.sync();
+  for (u64 row = tid; row < n; row += stride) index_insert_row(ix, row);
 }
 #endif
 
