@@ -292,11 +292,20 @@ extern "C" int emu_check_evm_x(const uint64_t* steps, uint64_t n_steps, const ui
   IndexStore s8, s9;
   IndexDev wd_ix = build_index(g_emu_wd, g_emu_n_wd, 4, wk, 1, ch, s8);
   t.wd = wd_ix.tab;
-  t.rw_rwc = build_index((const u64*)rw, n_rw, 14, wk, 1, ch, s9);  // same storage choice as t.rw (same matrix)
-  t.rw_rwc.tab = t.rw.tab;
+  Store ws;
+  WitnessDev w = make_witness(ws, (const u64*)steps, n_steps, 13, nullptr);
+  // as api.cu:check_evm, the indexes and constants of es_needs only for the states of the checked steps; otherwise an
+  // index without rows (every lookup there is unsat) and zeroed block stats, so that a missing needs bit fails here too
+  unsigned needs = 0;
+  for (u64 i = row_begin; i < row_end; i++) {
+    const Fr cs = wcell(w, S_STATE, i);
+    if (fr_fits64(cs) && cs.l[0] < ZK_ES_COUNT) needs |= es_needs((int)cs.l[0]);
+  }
+  t.rw_rwc = build_index((const u64*)rw, needs & RW_BY_COUNTER ? n_rw : 0, 14, wk, 1, ch, s9);
+  if (needs & RW_BY_COUNTER) t.rw_rwc.tab = t.rw.tab;  // same storage choice as t.rw (same matrix)
   IndexStore s10;
-  t.bytecode4 = build_index((const u64*)bytecode, n_bytecode, 6, k4, 4, ch, s10);  // bytecode_lookup_pair (evm_err.cuh)
-  t.bytecode4.tab = t.bytecode.tab;
+  t.bytecode4 = build_index((const u64*)bytecode, needs & BYTECODE_PAIR ? n_bytecode : 0, 6, k4, 4, ch, s10);  // evm_err.cuh
+  if (needs & BYTECODE_PAIR) t.bytecode4.tab = t.bytecode.tab;
   g_emu_tx = g_emu_block = nullptr;
   g_emu_n_tx = g_emu_n_block = 0;
   g_emu_tx_flags = g_emu_block_flags = nullptr;
@@ -311,14 +320,14 @@ extern "C" int emu_check_evm_x(const uint64_t* steps, uint64_t n_steps, const ui
   t.resp_bitmap = fxc.bitmap.data();
   BlockStats stats;  // k_evm_block_stats, serially
   memset(&stats, 0, sizeof(stats));
-  for (u64 r = 0; r < t.tx.tab.n_rows; r++) block_stats_tx_row(t.tx, (u32)r, &stats);
-  for (u64 r = 0; r < t.wd.n_rows; r++) block_stats_wd_row(t.wd, (u32)r, &stats);
-  if (pos_enabled(t.rw) && t.rw.pos_kind == ZK_POS_DENSE) stats.max_rws = (u32)t.rw.tab.n_rows;
-  else
-    for (u64 r = 0; r < t.rw.tab.n_rows; r++) stats.max_rws += first_of_kind_ix(t.rw_rwc, (u32)r) ? 1 : 0;
+  if (needs & BLOCK_STATS) {
+    for (u64 r = 0; r < t.tx.tab.n_rows; r++) block_stats_tx_row(t.tx, (u32)r, &stats);
+    for (u64 r = 0; r < t.wd.n_rows; r++) block_stats_wd_row(t.wd, (u32)r, &stats);
+    if (pos_enabled(t.rw) && t.rw.pos_kind == ZK_POS_DENSE) stats.max_rws = (u32)t.rw.tab.n_rows;
+    else
+      for (u64 r = 0; r < t.rw.tab.n_rows; r++) stats.max_rws += first_of_kind_ix(t.rw_rwc, (u32)r) ? 1 : 0;
+  }
   t.stats = &stats;
-  Store ws;
-  WitnessDev w = make_witness(ws, (const u64*)steps, n_steps, 13, nullptr);
   ResultDev res;
   init_result(res, first_fail, fail_count, EV_N_CONSTRAINTS);
   Fr stack_pre[2];

@@ -127,9 +127,7 @@ struct zk_ctx {
   cudaStream_t evm_aux = nullptr;
   cudaEvent_t evm_fork_ev = nullptr, evm_join_ev = nullptr;
   int evm_tx_overlap = 1;  // env ZKCHECK_TX_OVERLAP at context creation ("0..." = in-line order)
-  int evm_occ[20] = {0};  // resident blocks per SM of the gate-program kernels (0 = not queried yet)
-  int prep_occ = 0;       // blocks per SM of k_index_prepare's cooperative grid (0 = not queried yet)
-  std::unordered_map<const void*, int> occ;  // same, row-circuit kernels (keyed by kernel)
+  std::unordered_map<const void*, int> occ;  // resident blocks per SM of each kernel launched with a persistent grid
   BlockStats* block_stats = nullptr;  // k_evm_block_stats output
   void* state_fold = nullptr;  // k_state_fold output: 64 bytes per resident state row
   size_t state_fold_cap = 0;
@@ -162,6 +160,14 @@ static size_t up32(size_t x) { return (x + 31) / 32 * 32; }
 static int fail_msg(zk_ctx* ctx, const std::string& m) {
   ctx->err = m;
   return -1;
+}
+// after `n` kernel launches: counts them, and reports a failed launch (a CUDA error, as CK) by the kernel's name
+static int launched(zk_ctx* ctx, const char* kernel, int n = 1) {
+  ctx->launches += n;
+  const cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) return 0;
+  ctx->err = std::string("launch of ") + kernel + ": " + cudaGetErrorString(e);
+  return -2;
 }
 
 extern "C" int zk_ctx_create(int device_ordinal, zk_ctx** out) {
@@ -507,9 +513,7 @@ extern "C" int zk_upload_bytecode_table_from_code(zk_ctx* ctx, uint64_t n_contra
   BytecodeSrc src{sg + s_code, sg + s_bits, (const u64*)(sg + s_off), (const u64*)(sg + s_hash), n_contracts, n_rows};
   const unsigned grid = (unsigned)std::min<u64>((n_rows + 255) / 256, (u64)ctx->sm_count * 16);
   k_bytecode_table_expand<<<grid, 256, 0, st>>>(src, (unsigned char*)m.dev, off[0], off[1], off[2], off[3], off[4], off[5]);
-  ctx->launches += 1;
-  CK(ctx, cudaGetLastError());
-  return 0;
+  return launched(ctx, "k_bytecode_table_expand");
 }
 
 // ------------------------------------------------------------------ Keccak-256 on the device
@@ -589,8 +593,7 @@ extern "C" int zk_keccak256_batch(zk_ctx* ctx, uint64_t n, const uint8_t* data, 
   int rc = keccak_stage(ctx, n, data, offsets, st, &job, &dig);
   if (rc) return rc;
   k_keccak256<<<(unsigned)n, 128, 0, st>>>(job, dig, nullptr, 0, 0, 0, 0, 0, Fr{{0, 0, 0, 0}});
-  ctx->launches++;
-  CK(ctx, cudaGetLastError());
+  if ((rc = launched(ctx, "k_keccak256"))) return rc;
   CK(ctx, cudaMemcpyAsync(digests, dig, n * 32, cudaMemcpyDeviceToHost, st));
   CK(ctx, cudaStreamSynchronize(st));
   return 0;
@@ -624,9 +627,7 @@ extern "C" int zk_assign_keccak_table(zk_ctx* ctx, uint64_t n, const uint8_t* da
   layout_canonical(m.off, m.width, 5, n);
   const Fr r_mont = fr_to_mont(ctx->chal[ZK_CHALLENGE_KECCAK]);
   k_keccak256<<<(unsigned)n, 128, 0, st>>>(job, dig, (unsigned char*)m.dev, m.off[0], m.off[1], m.off[2], m.off[3], m.off[4], r_mont);
-  ctx->launches++;
-  CK(ctx, cudaGetLastError());
-  return 0;
+  return launched(ctx, "k_keccak256");
 }
 
 // ------------------------------------------------------------------ witness assignment on the device (assign.cu)
@@ -676,9 +677,7 @@ static int run_seg_scan(zk_ctx* ctx, const SegHorner& s, Fr* chunk_val, Fr* seg_
   if (s.n_chunks == 0) return 0;
   k_seg_local<<<(unsigned)((s.n_chunks + 255) / 256), 256, 0, st>>>(s, chunk_val);
   k_seg_carry<<<(unsigned)((s.n_seg + 127) / 128), 128, 0, st>>>(s, chunk_val, seg_total);
-  ctx->launches += 2;
-  CK(ctx, cudaGetLastError());
-  return 0;
+  return launched(ctx, "k_seg_local / k_seg_carry", 2);
 }
 
 extern "C" int zk_assign_bytecode_circuit(zk_ctx* ctx, uint32_t k, uint64_t n_contracts, const uint8_t* code,
@@ -723,9 +722,7 @@ extern "C" int zk_assign_bytecode_circuit(zk_ctx* ctx, uint32_t k, uint64_t n_co
   if ((rc = run_seg_scan(ctx, a.s, chunk_val, nullptr, st))) return rc;
   k_assign_bytecode_rows<<<(unsigned)std::min<u64>((n_rows + 255) / 256, (u64)ctx->sm_count * 16), 256, 0, st>>>(a);
   if (n_chunks) k_assign_bytecode_rlc<<<(unsigned)((n_chunks + 255) / 256), 256, 0, st>>>(a, chunk_val);
-  ctx->launches += n_chunks ? 2 : 1;
-  CK(ctx, cudaGetLastError());
-  return 0;
+  return launched(ctx, "k_assign_bytecode_rows / k_assign_bytecode_rlc", n_chunks ? 2 : 1);
 }
 
 extern "C" int zk_assign_state_circuit(zk_ctx* ctx, uint64_t n_rows, const void* packed_ops, uint64_t total_bytes,
@@ -781,9 +778,7 @@ extern "C" int zk_assign_state_circuit(zk_ctx* ctx, uint64_t n_rows, const void*
   a.kbytes = (unsigned char*)m.dev + front + 10 * limb_stride;
   a.n_rows = n_rows, a.limb_stride = limb_stride, a.byte_stride = byte_stride;
   k_assign_state_derive<<<(unsigned)std::min<u64>((n_rows + 255) / 256, (u64)ctx->sm_count * 16), 256, 0, st>>>(a);
-  ctx->launches++;
-  CK(ctx, cudaGetLastError());
-  return 0;
+  return launched(ctx, "k_assign_state_derive");
 }
 
 extern "C" int zk_assign_copy_circuit(zk_ctx* ctx, uint64_t n_events, const uint64_t* events, const uint8_t* data,
@@ -833,9 +828,7 @@ extern "C" int zk_assign_copy_circuit(zk_ctx* ctx, uint64_t n_events, const uint
   Fr* seg_total = (Fr*)(sg + s_tot);
   if ((rc = run_seg_scan(ctx, a.s, chunk_val, seg_total, st))) return rc;
   k_assign_copy_rows<<<(unsigned)((n_chunks + 255) / 256), 256, 0, st>>>(a, chunk_val, seg_total);
-  ctx->launches++;
-  CK(ctx, cudaGetLastError());
-  return 0;
+  return launched(ctx, "k_assign_copy_rows");
 }
 
 extern "C" int64_t zk_resident_rows(zk_ctx* ctx, int circuit_id) {
@@ -883,6 +876,25 @@ static TableDev table_dev(const zk_ctx* ctx, int table_id) {
   }
   t.flags = (m.flags_rows == m.n_rows && m.n_rows) ? m.flags : nullptr;
   return t;
+}
+
+// blocks of `kernel` the device keeps resident at `threads` per block (occupancy x SMs), queried once per kernel
+template <class K>
+static u64 resident_blocks(zk_ctx* ctx, K kernel, int threads) {
+  const void* key = (const void*)kernel;
+  auto it = ctx->occ.find(key);
+  if (it == ctx->occ.end()) {
+    int occ = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, 0) != cudaSuccess || occ < 1) occ = 1;
+    it = ctx->occ.emplace(key, occ).first;
+  }
+  return (u64)it->second * ctx->sm_count;
+}
+// persistent grid: enough blocks for one thread per item, but no more than the device keeps resident; threads
+// walk the items with a grid stride
+template <class K>
+static unsigned grid_persistent(zk_ctx* ctx, K kernel, int threads, u64 n_items) {
+  return (unsigned)std::max<u64>(1, std::min<u64>((n_items + threads - 1) / threads, resident_blocks(ctx, kernel, threads)));
 }
 
 // Returns the device descriptor of the index of `table_id` on `key_cols`, building it on
@@ -965,14 +977,9 @@ static int ensure_index(zk_ctx* ctx, int table_id, const u32* key_cols, u32 n_ke
     // verify pass, positional flag and (only if the table is not positional) the hash index: one cooperative launch
     // (lookup.cuh k_index_prepare).  Its grid stays within the blocks the device keeps resident, and a small table
     // gets a small grid.
-    if (!ctx->prep_occ) {
-      int occ = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_index_prepare, 256, 0) != cudaSuccess || occ < 1) occ = 1;
-      ctx->prep_occ = occ;
-    }
-    const u64 max_grid = (u64)ctx->prep_occ * ctx->sm_count;
+    const u64 max_grid = resident_blocks(ctx, k_index_prepare, 256);
     const u64 work = std::max<u64>(t.n_rows, ix->pos_kind == ZK_POS_RUNS ? (u64)ZK_HEADS_CAP : 0);  // + clearing the heads
-    const unsigned grid = (unsigned)std::max<u64>(1, std::min<u64>((work + 1023) / 1024, max_grid));
+    const unsigned grid = grid_persistent(ctx, k_index_prepare, 256, (work + 3) / 4);  // 4 rows per thread
     IndexPrep prep{nullptr, nullptr, nullptr, 0};
     if (ix->pos_kind != ZK_POS_NONE) {
       if (!ix->pos_part || ix->pos_part_cap < grid) {
@@ -990,8 +997,10 @@ static int ensure_index(zk_ctx* ctx, int table_id, const u32* key_cols, u32 n_ke
       d.pos_ok = ix->pos_flag;
     }
     void* args[] = {(void*)&d, (void*)&prep};
-    CK(ctx, cudaLaunchCooperativeKernel((const void*)k_index_prepare, dim3(grid), dim3(256), args, 0, st));
-    ctx->launches += 1;
+    // a failed launch is also the last CUDA error, which launched() reports
+    (void)cudaLaunchCooperativeKernel((const void*)k_index_prepare, dim3(grid), dim3(256), args, 0, st);
+    const int rc = launched(ctx, "k_index_prepare");
+    if (rc) return rc;
   } else if (!ix->empty_ready) {  // an empty table: clear the (minimum-size) slot array once
     CK(ctx, cudaMemsetAsync(ix->slots, 0xFF, cap * sizeof(u64), st));
   }
@@ -1049,20 +1058,6 @@ static bool is_canonical(const Matrix& m) {
     if (m.width[c] != 32) return false;
   return true;
 }
-// persistent grid: no more blocks than the device keeps resident (occupancy x SMs); threads walk the
-// rows with a grid stride
-template <class K>
-static unsigned grid_persistent(zk_ctx* ctx, K kernel, int threads, u64 n_items) {
-  const void* key = (const void*)kernel;
-  auto it = ctx->occ.find(key);
-  if (it == ctx->occ.end()) {
-    int occ = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, 0) != cudaSuccess || occ < 1) occ = 1;
-    it = ctx->occ.emplace(key, occ).first;
-  }
-  const u64 want = (n_items + threads - 1) / threads;
-  return (unsigned)std::max<u64>(1, std::min<u64>(want, (u64)it->second * ctx->sm_count));
-}
 static int check_bytecode(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStream_t st) {
   const u32 pk[2] = {0, 1}, kk[5] = {0, 1, 2, 3, 4};
   IndexDev push_ix, kec_ix;
@@ -1077,9 +1072,7 @@ static int check_bytecode(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cuda
     k_check_bytecode<L_CANON><<<grid_persistent(ctx, k_check_bytecode<L_CANON>, 256, n), 256, 0, st>>>(witness_dev(m), rg, push_ix, kec_ix, r_mont, res);
   else
     k_check_bytecode<L_ANY><<<grid_persistent(ctx, k_check_bytecode<L_ANY>, 256, n), 256, 0, st>>>(witness_dev(m), rg, push_ix, kec_ix, r_mont, res);
-  ctx->launches++;
-  CK(ctx, cudaGetLastError());
-  return 0;
+  return launched(ctx, "k_check_bytecode");
 }
 
 static int check_tx(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStream_t st, bool sig = false) {
@@ -1093,9 +1086,7 @@ static int check_tx(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStream
   const Fr r_mont = fr_to_mont(ctx->chal[ZK_CHALLENGE_KECCAK]);
   if (sig) k_check_sig<<<grid, 128, 0, st>>>(witness_dev(ctx->circ[ZK_CIRCUIT_SIG]), rg, kec_ix, r_mont, res);
   else k_check_tx<<<grid, 128, 0, st>>>(witness_dev(ctx->circ[ZK_CIRCUIT_TX]), rg, kec_ix, r_mont, res);
-  ctx->launches++;
-  CK(ctx, cudaGetLastError());
-  return 0;
+  return launched(ctx, sig ? "k_check_sig" : "k_check_tx");
 }
 
 static int check_exp(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStream_t st) {
@@ -1107,9 +1098,7 @@ static int check_exp(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStrea
   const u64 n = rg.row_end - rg.row_begin;
   if (is_canonical(m)) k_check_exp<L_CANON><<<grid_persistent(ctx, k_check_exp<L_CANON>, 128, n), 128, 0, st>>>(witness_dev(m), rg, res);
   else k_check_exp<L_ANY><<<grid_persistent(ctx, k_check_exp<L_ANY>, 128, n), 128, 0, st>>>(witness_dev(m), rg, res);
-  ctx->launches++;
-  CK(ctx, cudaGetLastError());
-  return 0;
+  return launched(ctx, "k_check_exp");
 }
 
 static int check_pi(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStream_t st) {
@@ -1127,9 +1116,7 @@ static int check_pi(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStream
   const u64 n = rg.row_end - rg.row_begin;
   if (is_canonical(m)) k_check_pi<L_CANON><<<grid_persistent(ctx, k_check_pi<L_CANON>, 256, n), 256, 0, st>>>(witness_dev(m), rg, kec_ix, gas_ix, pp, res);
   else k_check_pi<L_ANY><<<grid_persistent(ctx, k_check_pi<L_ANY>, 256, n), 256, 0, st>>>(witness_dev(m), rg, kec_ix, gas_ix, pp, res);
-  ctx->launches++;
-  CK(ctx, cudaGetLastError());
-  return 0;
+  return launched(ctx, "k_check_pi");
 }
 
 static int check_state(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStream_t st) {
@@ -1158,9 +1145,7 @@ static int check_state(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStr
     k_state_fold<L_ANY><<<grid_persistent(ctx, k_state_fold<L_ANY>, 256, m.n_rows), 256, 0, st>>>(wd, fold);
     k_check_state<L_ANY><<<grid_persistent(ctx, k_check_state<L_ANY>, 128, n), 128, 0, st>>>(wd, rg, mpt, res, fold);
   }
-  ctx->launches += 2;
-  CK(ctx, cudaGetLastError());
-  return 0;
+  return launched(ctx, "k_state_fold / k_check_state", 2);
 }
 
 static int check_copy(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStream_t st) {
@@ -1194,9 +1179,7 @@ static int check_copy(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStre
     k_check_copy_small<L_ANY><<<grid_persistent(ctx, k_check_copy_small<L_ANY>, 128, n), 128, 0, st>>>(witness_dev(m), rg, t, r_mont, res, slow);
     k_check_copy_general<L_ANY><<<g_general, 128, 0, st>>>(witness_dev(m), rg, t, r_mont, res, slow);
   }
-  ctx->launches += 2;
-  CK(ctx, cudaGetLastError());
-  return 0;
+  return launched(ctx, "k_check_copy_small / k_check_copy_general", 2);
 }
 
 // the narrow instances of the hot EVM kernels (evm.cu StepCtx::narrow) apply when the resident step matrix, rw table
@@ -1218,7 +1201,7 @@ static int check_evm(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStrea
   const Matrix& m = ctx->circ[ZK_CIRCUIT_EVM];
   if (rg.row_end + 1 > m.n_rows) return fail_msg(ctx, "EVM steps [b,e) need step e resident (rotation +1)");
   const u32 k5[5] = {0, 1, 2, 3, 4}, k4[4] = {0, 1, 2, 3};
-  EvmTables t;
+  EvmTables t{};
   int rc;
   if ((rc = ensure_index(ctx, ZK_TABLE_BYTECODE, k5, 5, st, &t.bytecode, ZK_POS_RUNS))) return rc;
   if ((rc = ensure_index(ctx, ZK_TABLE_RW, k5, 5, st, &t.rw, ZK_POS_DENSE))) return rc;
@@ -1240,13 +1223,12 @@ static int check_evm(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStrea
     CK(ctx, cudaMemsetAsync(ctx->resp_bitmap, 0, ZK_RESP_BITMAP_WORDS * sizeof(u32), st));
     if (t.fixed.tab.n_rows) {
       k_fixed_resp_bitmap<<<(unsigned)((t.fixed.tab.n_rows + 255) / 256), 256, 0, st>>>(t.fixed.tab, ctx->resp_bitmap);
-      ctx->launches++;
+      if ((rc = launched(ctx, "k_fixed_resp_bitmap"))) return rc;
     }
     ctx->resp_bitmap_version = ctx->tab[ZK_TABLE_FIXED].version;
   }
   t.resp_bitmap = ctx->resp_bitmap;
   t.wd = table_dev(ctx, ZK_TABLE_WITHDRAWAL);
-  t.stats = nullptr;
   if ((rc = mark_indexes_ready(ctx))) return rc;
   const u64 n = rg.row_end - rg.row_begin;
   // counting sort of the steps by execution state (k_evm_classify + k_evm_scatter), then one kernel
@@ -1280,124 +1262,79 @@ static int check_evm(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStrea
 #endif
   if (evm_narrow(ctx)) k_evm_classify<1><<<(unsigned)((n + ZK_CLASSIFY_THREADS - 1) / ZK_CLASSIFY_THREADS), ZK_CLASSIFY_THREADS, 0, st>>>(wd, rg, t, res, so);
   else k_evm_classify<0><<<sort_grid, 1024, 0, st>>>(wd, rg, t, res, so);
-  {
-    cudaError_t e_ = cudaGetLastError();
-    if (e_ != cudaSuccess) return fail_msg(ctx, std::string("launch of k_evm_classify: ") + cudaGetErrorString(e_));
-  }
+  if ((rc = launched(ctx, "k_evm_classify"))) return rc;
   CK(ctx, cudaEventRecord(ctx->evm_hist_ev, st));  // the histogram is in host memory once k_evm_classify is complete
   k_evm_scatter<<<sort_grid, 1024, 0, st>>>(so, (u32)n);
-  ctx->launches += 2;
-  {
-    cudaError_t e_ = cudaGetLastError();
-    if (e_ != cudaSuccess) return fail_msg(ctx, std::string("launch of k_evm_scatter: ") + cudaGetErrorString(e_));
-  }
+  if ((rc = launched(ctx, "k_evm_scatter"))) return rc;
   // the histogram decides which groups run and how large their grids are; the device keeps working on
   // the scatter meanwhile
   CK(ctx, cudaEventSynchronize(ctx->evm_hist_ev));
   const u32* hist = ctx->evm_hist_host;
   const bool pos = hist[ZK_EVM_NB] != 0;
   u64 group_n[KG_COUNT] = {0};
+  unsigned needs = 0;  // es_needs of the states present
   for (int b = 0; b < ZK_EVM_NB; b++) {
+    if (!hist[b]) continue;
     const int g = es_group(b);
     if (g >= 0) group_n[g] += hist[b];
+    needs |= es_needs(b);
   }
-  // transaction-level steps (BeginTx / EndTx / EndBlock) look rw rows up by other column subsets: a dense rw
-  // table serves them by position, otherwise through an index on rw_counter alone, built only now that such
-  // steps are known to exist; EndBlock also needs the table-derived constants
-  const u64 n_tx_level = (u64)hist[ZK_ES_BeginTx] + hist[ZK_ES_EndTx] + hist[ZK_ES_EndBlock] + hist[ZK_ES_SELFBALANCE] +
-                         hist[ZK_ES_BALANCE] + hist[ZK_ES_EXTCODEHASH] + hist[ZK_ES_EXTCODESIZE] + hist[ZK_ES_ErrorOutOfGasAccountAccess] +
-                         hist[ZK_ES_EXTCODECOPY] + hist[ZK_ES_ErrorOutOfGasMemoryCopy] + hist[ZK_ES_SLOAD] + hist[ZK_ES_SSTORE] +
-                         hist[ZK_ES_CALLDATALOAD] + hist[ZK_ES_LOG] + hist[ZK_ES_ErrorWriteProtection] + hist[ZK_ES_ErrorMaxCodeSizeExceeded] +
-                         hist[ZK_ES_ErrorOutOfGasCodeStore] + hist[ZK_ES_ErrorInvalidCreationCode] + hist[ZK_ES_RETURN] + hist[ZK_ES_ErrorOutOfGasCall] + hist[ZK_ES_CALL_OP] +
-                         hist[ZK_ES_CREATE] + hist[ZK_ES_CREATE2] + hist[ZK_ES_ErrorOutOfGasSloadSstore] + hist[ZK_ES_ErrorOutOfGasCREATE] +
-                         hist[ZK_ES_ErrorOutOfGasPrecompile] + hist[ZK_ES_ErrorGasUintOverflow];
-  if (hist[ZK_ES_ErrorInvalidJump] && !pos) {  // bytecode_lookup_pair: the index without is_code
-    const u32 k4b[4] = {0, 1, 2, 3};
-    if ((rc = ensure_index(ctx, ZK_TABLE_BYTECODE, k4b, 4, st, &t.bytecode4))) return rc;
-  }
-  if (n_tx_level) {
+  // positional tables serve every lookup by position; otherwise the extra indexes are built now that steps needing
+  // them are known to exist
+  if ((needs & BYTECODE_PAIR) && !pos && (rc = ensure_index(ctx, ZK_TABLE_BYTECODE, k4, 4, st, &t.bytecode4))) return rc;
+  if (needs & RW_BY_COUNTER) {
     const u32 k1[1] = {0};
     if (!pos && (rc = ensure_index(ctx, ZK_TABLE_RW, k1, 1, st, &t.rw_rwc))) return rc;
-    if (hist[ZK_ES_EndBlock]) {
-      if (!ctx->block_stats) CK(ctx, cudaMalloc(&ctx->block_stats, sizeof(BlockStats)));
-      CK(ctx, cudaMemsetAsync(ctx->block_stats, 0, sizeof(BlockStats), st));
-      const u64 rows = std::max<u64>(std::max<u64>(t.tx.tab.n_rows, t.wd.n_rows), pos ? 1 : t.rw.tab.n_rows);
-      k_evm_block_stats<<<(unsigned)std::max<u64>(1, std::min<u64>((rows + 255) / 256, (u64)ctx->sm_count * 8)), 256, 0, st>>>(t, ctx->block_stats);
-      ctx->launches++;
-      t.stats = ctx->block_stats;
-    }
   }
-  // persistent grids: at most the number of blocks the device keeps resident (occupancy x SMs), each
-  // thread walks its bucket with a grid stride
-  auto grid_for = [&](int slot, const void* kernel, u64 work_items, unsigned per_block) -> unsigned {
-    if (!ctx->evm_occ[slot]) {
-      int occ = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, 128, 0) != cudaSuccess || occ < 1) occ = 1;
-      ctx->evm_occ[slot] = occ;
-    }
-    const u64 want = (work_items + per_block - 1) / per_block;
-    return (unsigned)std::max<u64>(1, std::min<u64>(want, (u64)ctx->evm_occ[slot] * ctx->sm_count));
+  if (needs & BLOCK_STATS) {
+    if (!ctx->block_stats) CK(ctx, cudaMalloc(&ctx->block_stats, sizeof(BlockStats)));
+    CK(ctx, cudaMemsetAsync(ctx->block_stats, 0, sizeof(BlockStats), st));
+    const u64 rows = std::max<u64>(std::max<u64>(t.tx.tab.n_rows, t.wd.n_rows), pos ? 1 : t.rw.tab.n_rows);
+    k_evm_block_stats<<<(unsigned)std::max<u64>(1, std::min<u64>((rows + 255) / 256, (u64)ctx->sm_count * 8)), 256, 0, st>>>(t, ctx->block_stats);
+    if ((rc = launched(ctx, "k_evm_block_stats"))) return rc;
+    t.stats = ctx->block_stats;
+  }
+  // one kernel per non-empty group, on a persistent grid: each thread walks its buckets with a grid stride
+  using EvmKernel = void (*)(WitnessDev, CheckRange, EvmTables, ResultDev, EvmSort);
+  auto launch = [&](int g, EvmKernel kernel, const char* name, u64 threads_per_step, cudaStream_t s) {
+    if (!group_n[g]) return 0;
+    kernel<<<grid_persistent(ctx, kernel, 128, threads_per_step * group_n[g]), 128, 0, s>>>(wd, rg, t, res, so);
+    return launched(ctx, name);
   };
-#define ZK_LAUNCH_GROUP(slot, kernel, items, per_block) ZK_LAUNCH_GROUP_ON(st, slot, kernel, items, per_block)
-#define ZK_LAUNCH_GROUP_ON(stream_, slot, kernel, items, per_block)                            \
-  do {                                                                                         \
-    kernel<<<grid_for(slot, (const void*)kernel, items, per_block), 128, 0, stream_>>>(wd, rg, t, res, so); \
-    ctx->launches++;                                                                           \
-    {                                                                                          \
-      cudaError_t e_ = cudaGetLastError();                                                     \
-      if (e_ != cudaSuccess) return fail_msg(ctx, std::string("launch of " #kernel ": ") + cudaGetErrorString(e_)); \
-    }                                                                                          \
-  } while (0)
-  // narrow instances: positional tables AND every step column but the code hash, the rw table's key columns narrow
-  // (<= 8 bytes per row, Matrix::narrow_mask) AND the bytecode table in the layout k_bytecode_table_expand writes
-  const bool narrow = pos && evm_narrow(ctx);
+  // the hot groups' instances, indexed like k_evm_gadget's POS: 0 = hash indexes, 1 = positional rw + bytecode tables,
+  // 2 = positional and narrow: every step column but the code hash and the rw table's key columns stored in <= 8 bytes
+  // per row (Matrix::narrow_mask), and the bytecode table in the layout k_bytecode_table_expand writes
+  const int inst = pos ? (evm_narrow(ctx) ? 2 : 1) : 0;
+  static const EvmKernel k_push[3] = {k_evm_push_hash, k_evm_push_pos<0>, k_evm_push_pos<1>};
+  static const EvmKernel k_mul[3] = {k_evm_gadget<KG_MUL, 0>, k_evm_gadget<KG_MUL, 1>, k_evm_gadget<KG_MUL, 2>};
+  static const EvmKernel k_add[3] = {k_evm_gadget<KG_ADD, 0>, k_evm_gadget<KG_ADD, 1>, k_evm_gadget<KG_ADD, 2>};
+  static const EvmKernel k_pop[3] = {k_evm_gadget<KG_POP, 0>, k_evm_gadget<KG_POP, 1>, k_evm_gadget<KG_POP, 2>};
   // the transaction-level group first, on the auxiliary stream: its blocks take their places before the hot kernels'
   // persistent grids fill the device, and its long per-thread chains run underneath them
-  bool tx_forked = false;
-  if (group_n[KG_TX]) {
-    if (ctx->evm_tx_overlap) {
-      if (!ctx->evm_aux) {
-        CK(ctx, cudaStreamCreateWithFlags(&ctx->evm_aux, cudaStreamNonBlocking));
-        CK(ctx, cudaEventCreateWithFlags(&ctx->evm_fork_ev, cudaEventDisableTiming));
-        CK(ctx, cudaEventCreateWithFlags(&ctx->evm_join_ev, cudaEventDisableTiming));
-      }
-      CK(ctx, cudaEventRecord(ctx->evm_fork_ev, st));
-      CK(ctx, cudaStreamWaitEvent(ctx->evm_aux, ctx->evm_fork_ev, 0));
-      ZK_LAUNCH_GROUP_ON(ctx->evm_aux, 12, k_evm_group<KG_TX>, group_n[KG_TX], 128);
-      CK(ctx, cudaEventRecord(ctx->evm_join_ev, ctx->evm_aux));
-      tx_forked = true;
+  const bool tx_forked = group_n[KG_TX] && ctx->evm_tx_overlap;
+  if (tx_forked) {
+    if (!ctx->evm_aux) {
+      CK(ctx, cudaStreamCreateWithFlags(&ctx->evm_aux, cudaStreamNonBlocking));
+      CK(ctx, cudaEventCreateWithFlags(&ctx->evm_fork_ev, cudaEventDisableTiming));
+      CK(ctx, cudaEventCreateWithFlags(&ctx->evm_join_ev, cudaEventDisableTiming));
     }
+    CK(ctx, cudaEventRecord(ctx->evm_fork_ev, st));
+    CK(ctx, cudaStreamWaitEvent(ctx->evm_aux, ctx->evm_fork_ev, 0));
+    if ((rc = launch(KG_TX, k_evm_group<KG_TX>, "k_evm_group<KG_TX>", 1, ctx->evm_aux))) return rc;
+    CK(ctx, cudaEventRecord(ctx->evm_join_ev, ctx->evm_aux));
   }
-  if (group_n[KG_PUSH]) {
-    if (narrow) ZK_LAUNCH_GROUP(13, k_evm_push_pos<1>, group_n[KG_PUSH], 128);
-    else if (pos) ZK_LAUNCH_GROUP(0, k_evm_push_pos<0>, group_n[KG_PUSH], 128);
-    else ZK_LAUNCH_GROUP(1, k_evm_push_hash, group_n[KG_PUSH], 8);  // half a warp per step
-  }
-  if (group_n[KG_MUL]) {
-    if (narrow) ZK_LAUNCH_GROUP(14, (k_evm_gadget<KG_MUL, 2>), group_n[KG_MUL], 128);
-    else if (pos) ZK_LAUNCH_GROUP(2, (k_evm_gadget<KG_MUL, 1>), group_n[KG_MUL], 128);
-    else ZK_LAUNCH_GROUP(3, (k_evm_gadget<KG_MUL, 0>), group_n[KG_MUL], 128);
-  }
-  if (group_n[KG_ADD]) {
-    if (narrow) ZK_LAUNCH_GROUP(15, (k_evm_gadget<KG_ADD, 2>), group_n[KG_ADD], 128);
-    else if (pos) ZK_LAUNCH_GROUP(4, (k_evm_gadget<KG_ADD, 1>), group_n[KG_ADD], 128);
-    else ZK_LAUNCH_GROUP(5, (k_evm_gadget<KG_ADD, 0>), group_n[KG_ADD], 128);
-  }
-  if (group_n[KG_POP]) {
-    if (narrow) ZK_LAUNCH_GROUP(16, (k_evm_gadget<KG_POP, 2>), group_n[KG_POP], 128);
-    else if (pos) ZK_LAUNCH_GROUP(6, (k_evm_gadget<KG_POP, 1>), group_n[KG_POP], 128);
-    else ZK_LAUNCH_GROUP(7, (k_evm_gadget<KG_POP, 0>), group_n[KG_POP], 128);
-  }
-  if (group_n[KG_SIMPLE]) ZK_LAUNCH_GROUP(8, k_evm_group<KG_SIMPLE>, group_n[KG_SIMPLE], 128);
-  if (group_n[KG_BYTES32]) ZK_LAUNCH_GROUP(9, k_evm_group<KG_BYTES32>, group_n[KG_BYTES32], 128);
-  if (group_n[KG_COPY]) ZK_LAUNCH_GROUP(10, k_evm_group<KG_COPY>, group_n[KG_COPY], 128);
-  if (group_n[KG_WIDE]) ZK_LAUNCH_GROUP(11, k_evm_group<KG_WIDE>, group_n[KG_WIDE], 128);
-  if (group_n[KG_TX] && !tx_forked) ZK_LAUNCH_GROUP(12, k_evm_group<KG_TX>, group_n[KG_TX], 128);
-  if (group_n[KG_ARITH]) ZK_LAUNCH_GROUP(17, k_evm_group<KG_ARITH>, group_n[KG_ARITH], 128);
+  // k_evm_push_hash takes half a warp per step
+  if ((rc = launch(KG_PUSH, k_push[inst], inst ? "k_evm_push_pos" : "k_evm_push_hash", inst ? 1 : 16, st))) return rc;
+  if ((rc = launch(KG_MUL, k_mul[inst], "k_evm_gadget<KG_MUL>", 1, st))) return rc;
+  if ((rc = launch(KG_ADD, k_add[inst], "k_evm_gadget<KG_ADD>", 1, st))) return rc;
+  if ((rc = launch(KG_POP, k_pop[inst], "k_evm_gadget<KG_POP>", 1, st))) return rc;
+  if ((rc = launch(KG_SIMPLE, k_evm_group<KG_SIMPLE>, "k_evm_group<KG_SIMPLE>", 1, st))) return rc;
+  if ((rc = launch(KG_BYTES32, k_evm_group<KG_BYTES32>, "k_evm_group<KG_BYTES32>", 1, st))) return rc;
+  if ((rc = launch(KG_COPY, k_evm_group<KG_COPY>, "k_evm_group<KG_COPY>", 1, st))) return rc;
+  if ((rc = launch(KG_WIDE, k_evm_group<KG_WIDE>, "k_evm_group<KG_WIDE>", 1, st))) return rc;
+  if (!tx_forked && (rc = launch(KG_TX, k_evm_group<KG_TX>, "k_evm_group<KG_TX>", 1, st))) return rc;
+  if ((rc = launch(KG_ARITH, k_evm_group<KG_ARITH>, "k_evm_group<KG_ARITH>", 1, st))) return rc;
   if (tx_forked) CK(ctx, cudaStreamWaitEvent(st, ctx->evm_join_ev, 0));
-#undef ZK_LAUNCH_GROUP
-#undef ZK_LAUNCH_GROUP_ON
-  CK(ctx, cudaGetLastError());
   return 0;
 }
 
@@ -1583,9 +1520,7 @@ extern "C" int zk_allreduce_results(zk_ctx* ctx, int circuit_id, void* nccl_comm
   // ncclChar = 0 (nccl.h)
   if (g_nccl.all_gather(r.first_fail, ctx->gather, rank_bytes, 0, nccl_comm, st)) return fail_msg(ctx, "ncclAllGather failed");
   k_reduce_results<<<(r.n + 255) / 256, 256, 0, st>>>(ctx->gather, rank_bytes, count_off, world, r.n, r.first_fail, r.fail_count);
-  ctx->launches++;
-  CK(ctx, cudaGetLastError());
-  return 0;
+  return launched(ctx, "k_reduce_results");
 }
 
 // ------------------------------------------------------------------ introspection

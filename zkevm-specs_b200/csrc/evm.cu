@@ -6,10 +6,9 @@
 // step_state_transition_in_same_context (instruction.py:365-394, 206-264).
 // Hot gate programs (a kernel each): ADD/SUB (execution/add_sub.py:5-24), MUL/DIV/MOD
 // (mul_div_mod.py:6-71 with mul_add_words instruction.py:599-632 and compare_word :453-463), PUSH
-// (push.py:6-33), POP (pop.py:4-14).  Rare gate programs (k_evm_misc, one thread per step, out-of-line
-// lookups): SHA3, CALLDATACOPY, MEMORY, STOP with restore-to-caller-context, MSIZE, GAS, ISZERO, CMP, JUMP,
-// JUMPI, CALLER, CALLVALUE, CALLDATASIZE, ADDRESS, RETURNDATASIZE, CODESIZE, BITWISE, NOT, BYTE, SCMP,
-// SIGNEXTEND, BlockCtx, ORIGIN, GASPRICE, SHL_SHR (their execution/*.py files, cited at each program).
+// (push.py:6-33), POP (pop.py:4-14).  Every other gate program runs in the group kernel k_evm_group<G>, one
+// thread per step with out-of-line lookups (their execution/*.py files, cited at each program); the table
+// ZK_EVM_GATE_PROGRAMS below lists every state with a gate program and its group.
 // Every lookup() of the reference (table.py:864-884, a linear scan over a Python set) is either a
 // positional lookup on a verified-regular table or a probe of a device hash index (lookup.cuh).
 //
@@ -32,29 +31,140 @@ enum { S_STATE, S_RWC, S_CALL_ID, S_IS_ROOT, S_IS_CREATE, S_HASH_LO, S_HASH_HI, 
 enum { B_HASH_LO, B_HASH_HI, B_TAG, B_INDEX, B_ISCODE, B_VALUE };
 enum { R_RWC, R_RW, R_TAG, R_ID, R_ADDR, R_FIELD, R_KEY_LO, R_KEY_HI, R_VAL_LO, R_VAL_HI };
 
-// execution states with a gate program in this build (others: EV_UNSUPPORTED_STATE)
-#define ZK_ES_BUILT_LIST(X)                                                                                            \
-  X(ZK_ES_ADD) X(ZK_ES_MUL) X(ZK_ES_PUSH) X(ZK_ES_POP) X(ZK_ES_SHA3) X(ZK_ES_CALLDATACOPY) X(ZK_ES_STOP) X(ZK_ES_MEMORY)  \
-  X(ZK_ES_MSIZE) X(ZK_ES_GAS) X(ZK_ES_ISZERO) X(ZK_ES_CMP) X(ZK_ES_JUMP) X(ZK_ES_JUMPI) X(ZK_ES_CALLER) X(ZK_ES_CALLVALUE) \
-  X(ZK_ES_CALLDATASIZE) X(ZK_ES_ADDRESS) X(ZK_ES_RETURNDATASIZE) X(ZK_ES_CODESIZE) X(ZK_ES_BITWISE) X(ZK_ES_NOT)         \
-  X(ZK_ES_BYTE) X(ZK_ES_SCMP) X(ZK_ES_SIGNEXTEND) X(ZK_ES_BlockCtx) X(ZK_ES_ORIGIN) X(ZK_ES_GASPRICE) X(ZK_ES_SHL_SHR)      \
-  X(ZK_ES_BeginTx) X(ZK_ES_EndTx) X(ZK_ES_EndBlock) X(ZK_ES_ErrorStack) X(ZK_ES_ErrorInvalidOpcode)                    \
-  X(ZK_ES_ErrorOutOfGasConstant) X(ZK_ES_ErrorInvalidJump) X(ZK_ES_SELFBALANCE) X(ZK_ES_ErrorOutOfGasSHA3)                  \
-  X(ZK_ES_ErrorOutOfGasStaticMemoryExpansion) X(ZK_ES_ErrorOutOfGasDynamicMemoryExpansion) X(ZK_ES_ErrorOutOfGasLOG)       \
-  X(ZK_ES_ErrorOutOfGasEXP) X(ZK_ES_ErrorReturnDataOutOfBound) X(ZK_ES_BALANCE) X(ZK_ES_EXTCODEHASH) X(ZK_ES_EXTCODESIZE)          \
-  X(ZK_ES_ErrorOutOfGasAccountAccess) X(ZK_ES_CODECOPY) X(ZK_ES_RETURNDATACOPY) X(ZK_ES_EXTCODECOPY) X(ZK_ES_ErrorOutOfGasMemoryCopy) \
-  X(ZK_ES_ADDMOD) X(ZK_ES_MULMOD) X(ZK_ES_SDIV_SMOD) X(ZK_ES_SAR) X(ZK_ES_SLOAD) X(ZK_ES_SSTORE) X(ZK_ES_CALLDATALOAD) \
-  X(ZK_ES_LOG) X(ZK_ES_ErrorWriteProtection) X(ZK_ES_BLOCKHASH) X(ZK_ES_EXP) \
-  X(ZK_ES_ErrorMaxCodeSizeExceeded) X(ZK_ES_ErrorOutOfGasCodeStore) X(ZK_ES_ErrorInvalidCreationCode) X(ZK_ES_RETURN) X(ZK_ES_ErrorOutOfGasCall) X(ZK_ES_CALL_OP) \
-  X(ZK_ES_CREATE) X(ZK_ES_CREATE2) X(ZK_ES_ErrorOutOfGasSloadSstore) X(ZK_ES_ErrorOutOfGasCREATE) X(ZK_ES_ErrorOutOfGasPrecompile) \
-  X(ZK_ES_ErrorGasUintOverflow)
+// ---- gate programs --------------------------------------------------------------------------
+// One kernel per GROUP of gate programs with similar register needs; inside a group kernel every
+// execution state has its own bucket of steps, so warps run one gate program (k_evm_classify /
+// k_evm_scatter sort the steps by state).  The host launches a group only when one of its buckets is
+// non-empty (check_evm reads the histogram back).  ADD / MUL / PUSH / POP are the hot groups, each with
+// kernels of its own (k_evm_gadget, k_evm_push_*); the others run in k_evm_group<G>.
+enum { KG_ADD, KG_MUL, KG_PUSH, KG_POP, KG_SIMPLE, KG_BYTES32, KG_COPY, KG_WIDE, KG_TX, KG_ARITH, KG_COUNT };
+// what a gate program reads beyond the step matrix and the indexes every check builds; the host builds these only
+// when a step of such a state is present (api.cu:check_evm, tests/emu)
+enum : unsigned {
+  RW_BY_COUNTER = 1,  // rw rows by rw_counter plus other columns (rw_lookup_m): EvmTables::rw_rwc unless the rw table is dense
+  BYTECODE_PAIR = 2,  // bytecode rows without is_code (bytecode_pair_m): EvmTables::bytecode4 unless the table is positional
+  BLOCK_STATS = 4,    // EvmTables::stats (k_evm_block_stats)
+};
+// Every execution state with a gate program in this build, one row each: X(state, needs, call), in one list per group
+// (ZK_EVM_GROUPS pairs each list with its group).  `call` runs the gate program of a rare group's step `s` (StepCtx)
+// under the check's ZK_FLAG_EVM_* `flags`; the hot groups' rows name none.  S(state, needs): the state runs the gate
+// program of the row after it, as one case body of run_group's switch (a second call site changes the register
+// allocation of k_evm_group<KG_TX>, which sits at the 255-register limit).  ES_BUILT (other states fail with
+// EV_UNSUPPORTED_STATE), es_group, the switch of run_group<G> and es_needs all follow from these rows, so a new gate
+// program is one row.
+#define ZK_GATES_ADD(X, S) X(ZK_ES_ADD, 0, )
+#define ZK_GATES_MUL(X, S) X(ZK_ES_MUL, 0, )
+#define ZK_GATES_PUSH(X, S) X(ZK_ES_PUSH, 0, )
+#define ZK_GATES_POP(X, S) X(ZK_ES_POP, 0, )
+#define ZK_GATES_SIMPLE(X, S)                                                                        \
+  X(ZK_ES_MSIZE, 0, gadget_msize(s, true))                                                           \
+  X(ZK_ES_GAS, 0, gadget_gas(s, true))                                                               \
+  X(ZK_ES_ISZERO, 0, gadget_iszero(s, true))                                                         \
+  X(ZK_ES_CMP, 0, gadget_cmp(s, true))                                                               \
+  X(ZK_ES_JUMP, 0, gadget_jump(s, true))                                                             \
+  X(ZK_ES_JUMPI, 0, gadget_jumpi(s, true))                                                           \
+  X(ZK_ES_CALLER, 0, gadget_cc_push(s, true, 0x33, ZK_CC_CallerAddress, true))                       \
+  X(ZK_ES_CALLVALUE, 0, gadget_cc_push(s, true, 0x34, ZK_CC_Value, true))                            \
+  X(ZK_ES_CALLDATASIZE, 0, gadget_cc_push(s, true, 0x36, ZK_CC_CallDataLength, false))               \
+  X(ZK_ES_ADDRESS, 0, gadget_cc_push(s, true, 0x30, ZK_CC_CalleeAddress, true))                      \
+  X(ZK_ES_RETURNDATASIZE, 0, gadget_cc_push(s, true, 0x3d, ZK_CC_LastCalleeReturnDataLength, false)) \
+  X(ZK_ES_CODESIZE, 0, gadget_codesize(s, true))                                                     \
+  X(ZK_ES_BYTE, 0, gadget_byte(s, true))                                                             \
+  X(ZK_ES_SCMP, 0, gadget_scmp(s, true))                                                             \
+  X(ZK_ES_SIGNEXTEND, 0, gadget_signextend(s, true))                                                 \
+  X(ZK_ES_BlockCtx, 0, gadget_blockctx(s, true))                                                     \
+  X(ZK_ES_ORIGIN, 0, gadget_txctx(s, true, 0x32, ZK_TX_CallerAddress))                               \
+  X(ZK_ES_GASPRICE, 0, gadget_txctx(s, true, 0x3a, ZK_TX_GasPrice))
+#define ZK_GATES_BYTES32(X, S)                 \
+  X(ZK_ES_BITWISE, 0, gadget_bitwise(s, true)) \
+  X(ZK_ES_NOT, 0, gadget_not(s, true))         \
+  X(ZK_ES_MEMORY, 0, gadget_memory(s, true))
+#define ZK_GATES_COPY(X, S)                              \
+  X(ZK_ES_SHA3, 0, gadget_sha3(s, true))                 \
+  X(ZK_ES_CALLDATACOPY, 0, gadget_calldatacopy(s, true))
+#define ZK_GATES_WIDE(X, S)                    \
+  X(ZK_ES_SHL_SHR, 0, gadget_shl_shr(s, true))
+#define ZK_GATES_TX(X, S)                                                                                                       \
+  X(ZK_ES_STOP, 0, gadget_stop(s, true))                                                                                        \
+  X(ZK_ES_BeginTx, RW_BY_COUNTER, gadget_begin_tx(s, (flags & ZK_FLAG_EVM_FIRST_STEP) && s.row == 0))                           \
+  X(ZK_ES_EndTx, RW_BY_COUNTER, gadget_end_tx(s))                                                                               \
+  X(ZK_ES_EndBlock, RW_BY_COUNTER | BLOCK_STATS, gadget_end_block(s, (flags & ZK_FLAG_EVM_LAST_STEP) && s.i == s.w.n_rows - 2)) \
+  X(ZK_ES_ErrorStack, 0, gadget_error_stack(s))                                                                                 \
+  X(ZK_ES_ErrorInvalidOpcode, 0, gadget_error_invalid_opcode(s))                                                                \
+  X(ZK_ES_ErrorOutOfGasConstant, 0, gadget_error_oog_constant(s))                                                               \
+  X(ZK_ES_ErrorInvalidJump, BYTECODE_PAIR, gadget_error_invalid_jump(s))                                                        \
+  X(ZK_ES_SELFBALANCE, RW_BY_COUNTER, gadget_selfbalance(s))                                                                    \
+  X(ZK_ES_ErrorOutOfGasSHA3, 0, gadget_error_oog_sha3(s))                                                                       \
+  X(ZK_ES_ErrorOutOfGasStaticMemoryExpansion, 0, gadget_error_oog_static_memory(s))                                             \
+  X(ZK_ES_ErrorOutOfGasDynamicMemoryExpansion, 0, gadget_error_oog_dynamic_memory(s))                                           \
+  X(ZK_ES_ErrorOutOfGasLOG, 0, gadget_error_oog_log(s))                                                                         \
+  X(ZK_ES_ErrorOutOfGasEXP, 0, gadget_error_oog_exp(s))                                                                         \
+  X(ZK_ES_ErrorReturnDataOutOfBound, 0, gadget_error_return_data_oob(s))                                                        \
+  X(ZK_ES_BALANCE, RW_BY_COUNTER, gadget_account_access(s, 0x31))                                                               \
+  X(ZK_ES_EXTCODEHASH, RW_BY_COUNTER, gadget_account_access(s, 0x3f))                                                           \
+  X(ZK_ES_EXTCODESIZE, RW_BY_COUNTER, gadget_account_access(s, 0x3b))                                                           \
+  X(ZK_ES_ErrorOutOfGasAccountAccess, RW_BY_COUNTER, gadget_error_oog_account_access(s))                                        \
+  X(ZK_ES_CODECOPY, 0, gadget_codecopy(s))                                                                                      \
+  X(ZK_ES_RETURNDATACOPY, 0, gadget_returndatacopy(s))                                                                          \
+  X(ZK_ES_EXTCODECOPY, RW_BY_COUNTER, gadget_extcodecopy(s))                                                                    \
+  X(ZK_ES_ErrorOutOfGasMemoryCopy, RW_BY_COUNTER, gadget_error_oog_memory_copy(s))                                              \
+  X(ZK_ES_SLOAD, RW_BY_COUNTER, gadget_sload(s))                                                                                \
+  X(ZK_ES_SSTORE, RW_BY_COUNTER, gadget_sstore(s))                                                                              \
+  X(ZK_ES_CALLDATALOAD, RW_BY_COUNTER, gadget_calldataload(s))                                                                  \
+  X(ZK_ES_LOG, RW_BY_COUNTER, gadget_log(s))                                                                                    \
+  X(ZK_ES_ErrorWriteProtection, RW_BY_COUNTER, gadget_error_write_protection(s))                                                \
+  X(ZK_ES_BLOCKHASH, 0, gadget_blockhash(s))                                                                                    \
+  S(ZK_ES_ErrorMaxCodeSizeExceeded, RW_BY_COUNTER)                                                                              \
+  X(ZK_ES_ErrorOutOfGasCodeStore, RW_BY_COUNTER, gadget_error_code_store(s))                                                    \
+  X(ZK_ES_ErrorInvalidCreationCode, RW_BY_COUNTER, gadget_error_invalid_creation_code(s))                                       \
+  X(ZK_ES_RETURN, RW_BY_COUNTER, gadget_return_revert(s))                                                                       \
+  X(ZK_ES_ErrorOutOfGasCall, RW_BY_COUNTER, gadget_error_oog_call(s))                                                           \
+  X(ZK_ES_CALL_OP, RW_BY_COUNTER, gadget_callop(s))                                                                             \
+  S(ZK_ES_CREATE, RW_BY_COUNTER)                                                                                                \
+  X(ZK_ES_CREATE2, RW_BY_COUNTER, gadget_create(s))                                                                             \
+  X(ZK_ES_ErrorOutOfGasSloadSstore, RW_BY_COUNTER, gadget_error_oog_sload_sstore(s))                                            \
+  X(ZK_ES_ErrorOutOfGasCREATE, RW_BY_COUNTER, gadget_error_oog_create(s))                                                       \
+  X(ZK_ES_ErrorOutOfGasPrecompile, RW_BY_COUNTER, gadget_error_oog_precompile(s))                                               \
+  X(ZK_ES_ErrorGasUintOverflow, RW_BY_COUNTER, gadget_error_gas_uint_overflow(s))
+#define ZK_GATES_ARITH(X, S)                         \
+  X(ZK_ES_ADDMOD, 0, gadget_addmod_mulmod(s, false)) \
+  X(ZK_ES_MULMOD, 0, gadget_addmod_mulmod(s, true))  \
+  X(ZK_ES_SDIV_SMOD, 0, gadget_sdiv_smod(s))         \
+  X(ZK_ES_SAR, 0, gadget_sar(s))                     \
+  X(ZK_ES_EXP, 0, gadget_exp(s))
+#define ZK_EVM_GROUPS(Y)          \
+  Y(KG_ADD, ZK_GATES_ADD)         \
+  Y(KG_MUL, ZK_GATES_MUL)         \
+  Y(KG_PUSH, ZK_GATES_PUSH)       \
+  Y(KG_POP, ZK_GATES_POP)         \
+  Y(KG_SIMPLE, ZK_GATES_SIMPLE)   \
+  Y(KG_BYTES32, ZK_GATES_BYTES32) \
+  Y(KG_COPY, ZK_GATES_COPY)       \
+  Y(KG_WIDE, ZK_GATES_WIDE)       \
+  Y(KG_TX, ZK_GATES_TX)           \
+  Y(KG_ARITH, ZK_GATES_ARITH)
+
+__host__ __device__ constexpr unsigned es_needs(int st) {
+  switch (st) {
+#define ZK_X(state, needs, call) case state: return needs;
+#define ZK_S(state, needs) case state: return needs;
+#define ZK_Y(group, list) list(ZK_X, ZK_S)
+    ZK_EVM_GROUPS(ZK_Y)
+#undef ZK_Y
+#undef ZK_S
+#undef ZK_X
+    default: return 0;
+  }
+}
 struct EsBuiltTable {
   signed char v[ZK_ES_COUNT];
 };
 __host__ __device__ constexpr EsBuiltTable make_es_built() {
   EsBuiltTable t{};
-#define ZK_X(id) t.v[id] = 1;
-  ZK_ES_BUILT_LIST(ZK_X)
+#define ZK_X(state, ...) t.v[state] = 1;
+#define ZK_Y(group, list) list(ZK_X, ZK_X)
+  ZK_EVM_GROUPS(ZK_Y)
+#undef ZK_Y
 #undef ZK_X
   return t;
 }
@@ -97,11 +207,11 @@ struct EvmTables {
   IndexDev aux;       // step-aux side table (step row | aux_data lo, hi): StepState.aux_data of CREATE / CREATE2 (create.py:107), key =
                       // the step's row
   IndexDev bytecode4; // bytecode table keyed on (hash lo, hi, tag, index): bytecode_lookup_pair does not name is_code; only built
-                      // when an ErrorInvalidJump step exists and the bytecode table is not positional
-  IndexDev rw_rwc;    // rw table keyed on rw_counter alone: lookups that name other column subsets (evm_tx.cuh);
-                      // only built when a BeginTx / EndTx / EndBlock step exists and the rw table is not positional
+                      // when a step of a BYTECODE_PAIR state exists and the tables are not positional
+  IndexDev rw_rwc;    // rw table keyed on rw_counter alone: lookups that name other column subsets (rw_lookup_m); only
+                      // built when a step of an RW_BY_COUNTER state exists and the tables are not positional
   TableDev wd;        // withdrawal table (id, validator_id, address, amount), table.py:429-435
-  const struct BlockStats* stats;  // table-derived constants of EndBlock (k_evm_block_stats)
+  const struct BlockStats* stats;  // table-derived constants of EndBlock (k_evm_block_stats); only with a BLOCK_STATS state
   // ResponsibleOpcode rows of the fixed table (tag 13, aux 0) with state, opcode < 256 as a
   // 64 Kbit bitmap: bit (state << 8 | opcode).  Built from the uploaded fixed table
   // (k_fixed_resp_bitmap) and staged into shared memory by every EVM kernel.
@@ -942,9 +1052,9 @@ ZK_HD void gadget_pop(const StepCtx& s, bool live) {
   same_context(s, opcode, 1, fr_u64(1), fr_u64(1));
 }
 
-// Out-of-line copies of the shared lookups / epilogue for the RARE gate programs below: k_evm_misc holds
-// two dozen gate programs, and with every lookup inlined (hash path + positional path each) it took
-// ptxas 140 s to compile; the hot kernels keep the inlined forms.
+// Out-of-line copies of the shared lookups / epilogue for the RARE gate programs below: k_evm_group<KG_TX> alone
+// holds dozens of gate programs, and with every lookup inlined (hash path + positional path each) one kernel of two
+// dozen of them took ptxas 140 s to compile; the hot kernels keep the inlined forms.
 ZK_HD_NOINLINE int rw_lookup_ni(const StepCtx& s, bool live, const Fr& rwc, u64 rw, u64 tag, const Fr& id, const Fr& addr,
                                 Word2* value) {
   return rw_lookup(s, live, rwc, rw, tag, id, addr, value);
@@ -1721,138 +1831,34 @@ ZK_HD_NOINLINE void gadget_shl_shr(const StepCtx& s, bool live) {
 #include "evm_create.cuh"
 namespace zk {
 
-// ---- gate-program groups --------------------------------------------------------------------
-// One kernel per GROUP of gate programs with similar register needs; inside a group kernel every
-// execution state has its own bucket of steps, so warps run one gate program (k_evm_classify /
-// k_evm_scatter sort the steps by state).  The host launches a group only when one of its buckets is
-// non-empty (zk_check_async reads the histogram back).
-enum { KG_ADD, KG_MUL, KG_PUSH, KG_POP, KG_SIMPLE, KG_BYTES32, KG_COPY, KG_WIDE, KG_TX, KG_ARITH, KG_COUNT };
 __host__ __device__ constexpr int es_group(int st) {
   switch (st) {
-    case ZK_ES_ADD: return KG_ADD;
-    case ZK_ES_MUL: case ZK_BK_DIV: case ZK_BK_MOD: return KG_MUL;
-    case ZK_ES_PUSH: return KG_PUSH;
-    case ZK_ES_POP: return KG_POP;
-    case ZK_ES_MSIZE: case ZK_ES_GAS: case ZK_ES_ISZERO: case ZK_ES_CMP: case ZK_ES_JUMP: case ZK_ES_JUMPI:
-    case ZK_ES_CALLER: case ZK_ES_CALLVALUE: case ZK_ES_CALLDATASIZE: case ZK_ES_ADDRESS: case ZK_ES_RETURNDATASIZE:
-    case ZK_ES_CODESIZE: case ZK_ES_BYTE: case ZK_ES_SCMP: case ZK_ES_SIGNEXTEND: case ZK_ES_BlockCtx:
-    case ZK_ES_ORIGIN: case ZK_ES_GASPRICE: return KG_SIMPLE;
-    case ZK_ES_BITWISE: case ZK_ES_NOT: case ZK_ES_MEMORY: return KG_BYTES32;
-    case ZK_ES_SHA3: case ZK_ES_CALLDATACOPY: return KG_COPY;
-    case ZK_ES_SHL_SHR: return KG_WIDE;
-    case ZK_ES_ADDMOD: case ZK_ES_MULMOD: case ZK_ES_SDIV_SMOD: case ZK_ES_SAR: case ZK_ES_EXP: return KG_ARITH;
-    case ZK_ES_STOP: case ZK_ES_BeginTx: case ZK_ES_EndTx: case ZK_ES_EndBlock: case ZK_ES_ErrorStack:
-    case ZK_ES_ErrorInvalidOpcode: case ZK_ES_ErrorOutOfGasConstant: case ZK_ES_ErrorInvalidJump: case ZK_ES_SELFBALANCE:
-    case ZK_ES_ErrorOutOfGasSHA3: case ZK_ES_ErrorOutOfGasStaticMemoryExpansion: case ZK_ES_ErrorOutOfGasDynamicMemoryExpansion:
-    case ZK_ES_ErrorOutOfGasLOG: case ZK_ES_ErrorOutOfGasEXP: case ZK_ES_ErrorReturnDataOutOfBound:
-    case ZK_ES_BALANCE: case ZK_ES_EXTCODEHASH: case ZK_ES_EXTCODESIZE: case ZK_ES_ErrorOutOfGasAccountAccess:
-    case ZK_ES_CODECOPY: case ZK_ES_RETURNDATACOPY: case ZK_ES_EXTCODECOPY: case ZK_ES_ErrorOutOfGasMemoryCopy:
-    case ZK_ES_SLOAD: case ZK_ES_SSTORE: case ZK_ES_CALLDATALOAD: case ZK_ES_LOG: case ZK_ES_ErrorWriteProtection: case ZK_ES_BLOCKHASH:
-    case ZK_ES_ErrorMaxCodeSizeExceeded: case ZK_ES_ErrorOutOfGasCodeStore: case ZK_ES_ErrorInvalidCreationCode:
-    case ZK_ES_RETURN: case ZK_ES_ErrorOutOfGasCall: case ZK_ES_CALL_OP: case ZK_ES_CREATE: case ZK_ES_CREATE2:
-    case ZK_ES_ErrorOutOfGasSloadSstore: case ZK_ES_ErrorOutOfGasCREATE: case ZK_ES_ErrorOutOfGasPrecompile:
-    case ZK_ES_ErrorGasUintOverflow:
-      return KG_TX;
+#define ZK_X(state, ...) case state:
+#define ZK_Y(group, list) list(ZK_X, ZK_X) return group;
+    ZK_EVM_GROUPS(ZK_Y)
+#undef ZK_Y
+#undef ZK_X
+    case ZK_BK_DIV: case ZK_BK_MOD: return KG_MUL;  // buckets of MUL-state steps (k_evm_classify), not states
     default: return -1;
   }
 }
-// the rare gate programs of one group (st = execution state; other states: nothing)
+// the gate program of a rare group's step (st = its execution state; other states: nothing)
 // `flags`: ZK_FLAG_EVM_* of the check (BeginTx / EndBlock look at the first / last step rules, main.py:47-56)
 template <int G>
 ZK_HD void run_group(const StepCtx& s, int st, u32 flags) {
-  if constexpr (G == KG_SIMPLE) {
-    switch (st) {
-      case ZK_ES_MSIZE: gadget_msize(s, true); break;
-      case ZK_ES_GAS: gadget_gas(s, true); break;
-      case ZK_ES_ISZERO: gadget_iszero(s, true); break;
-      case ZK_ES_CMP: gadget_cmp(s, true); break;
-      case ZK_ES_JUMP: gadget_jump(s, true); break;
-      case ZK_ES_JUMPI: gadget_jumpi(s, true); break;
-      case ZK_ES_CALLER: gadget_cc_push(s, true, 0x33, ZK_CC_CallerAddress, true); break;
-      case ZK_ES_CALLVALUE: gadget_cc_push(s, true, 0x34, ZK_CC_Value, true); break;
-      case ZK_ES_CALLDATASIZE: gadget_cc_push(s, true, 0x36, ZK_CC_CallDataLength, false); break;
-      case ZK_ES_ADDRESS: gadget_cc_push(s, true, 0x30, ZK_CC_CalleeAddress, true); break;
-      case ZK_ES_RETURNDATASIZE: gadget_cc_push(s, true, 0x3d, ZK_CC_LastCalleeReturnDataLength, false); break;
-      case ZK_ES_CODESIZE: gadget_codesize(s, true); break;
-      case ZK_ES_BYTE: gadget_byte(s, true); break;
-      case ZK_ES_SCMP: gadget_scmp(s, true); break;
-      case ZK_ES_SIGNEXTEND: gadget_signextend(s, true); break;
-      case ZK_ES_BlockCtx: gadget_blockctx(s, true); break;
-      case ZK_ES_ORIGIN: gadget_txctx(s, true, 0x32, ZK_TX_CallerAddress); break;
-      case ZK_ES_GASPRICE: gadget_txctx(s, true, 0x3a, ZK_TX_GasPrice); break;
-      default: break;
-    }
-  } else if constexpr (G == KG_BYTES32) {
-    switch (st) {
-      case ZK_ES_BITWISE: gadget_bitwise(s, true); break;
-      case ZK_ES_NOT: gadget_not(s, true); break;
-      case ZK_ES_MEMORY: gadget_memory(s, true); break;
-      default: break;
-    }
-  } else if constexpr (G == KG_COPY) {
-    switch (st) {
-      case ZK_ES_SHA3: gadget_sha3(s, true); break;
-      case ZK_ES_CALLDATACOPY: gadget_calldatacopy(s, true); break;
-      default: break;
-    }
-  } else if constexpr (G == KG_WIDE) {
-    switch (st) {
-      case ZK_ES_SHL_SHR: gadget_shl_shr(s, true); break;
-      default: break;
-    }
-  } else if constexpr (G == KG_TX) {
-    switch (st) {
-      case ZK_ES_STOP: gadget_stop(s, true); break;
-      case ZK_ES_BeginTx: gadget_begin_tx(s, (flags & ZK_FLAG_EVM_FIRST_STEP) && s.row == 0); break;
-      case ZK_ES_EndTx: gadget_end_tx(s); break;
-      case ZK_ES_EndBlock: gadget_end_block(s, (flags & ZK_FLAG_EVM_LAST_STEP) && s.i == s.w.n_rows - 2); break;
-      case ZK_ES_ErrorStack: gadget_error_stack(s); break;
-      case ZK_ES_ErrorInvalidOpcode: gadget_error_invalid_opcode(s); break;
-      case ZK_ES_ErrorOutOfGasConstant: gadget_error_oog_constant(s); break;
-      case ZK_ES_ErrorInvalidJump: gadget_error_invalid_jump(s); break;
-      case ZK_ES_SELFBALANCE: gadget_selfbalance(s); break;
-      case ZK_ES_ErrorOutOfGasSHA3: gadget_error_oog_sha3(s); break;
-      case ZK_ES_ErrorOutOfGasStaticMemoryExpansion: gadget_error_oog_static_memory(s); break;
-      case ZK_ES_ErrorOutOfGasDynamicMemoryExpansion: gadget_error_oog_dynamic_memory(s); break;
-      case ZK_ES_ErrorOutOfGasLOG: gadget_error_oog_log(s); break;
-      case ZK_ES_ErrorOutOfGasEXP: gadget_error_oog_exp(s); break;
-      case ZK_ES_ErrorReturnDataOutOfBound: gadget_error_return_data_oob(s); break;
-      case ZK_ES_BALANCE: gadget_account_access(s, 0x31); break;
-      case ZK_ES_EXTCODEHASH: gadget_account_access(s, 0x3f); break;
-      case ZK_ES_EXTCODESIZE: gadget_account_access(s, 0x3b); break;
-      case ZK_ES_ErrorOutOfGasAccountAccess: gadget_error_oog_account_access(s); break;
-      case ZK_ES_CODECOPY: gadget_codecopy(s); break;
-      case ZK_ES_RETURNDATACOPY: gadget_returndatacopy(s); break;
-      case ZK_ES_EXTCODECOPY: gadget_extcodecopy(s); break;
-      case ZK_ES_ErrorOutOfGasMemoryCopy: gadget_error_oog_memory_copy(s); break;
-      case ZK_ES_SLOAD: gadget_sload(s); break;
-      case ZK_ES_SSTORE: gadget_sstore(s); break;
-      case ZK_ES_CALLDATALOAD: gadget_calldataload(s); break;
-      case ZK_ES_LOG: gadget_log(s); break;
-      case ZK_ES_ErrorWriteProtection: gadget_error_write_protection(s); break;
-      case ZK_ES_BLOCKHASH: gadget_blockhash(s); break;
-      case ZK_ES_ErrorMaxCodeSizeExceeded: case ZK_ES_ErrorOutOfGasCodeStore: gadget_error_code_store(s); break;
-      case ZK_ES_ErrorInvalidCreationCode: gadget_error_invalid_creation_code(s); break;
-      case ZK_ES_RETURN: gadget_return_revert(s); break;
-      case ZK_ES_ErrorOutOfGasCall: gadget_error_oog_call(s); break;
-      case ZK_ES_CALL_OP: gadget_callop(s); break;
-      case ZK_ES_CREATE: case ZK_ES_CREATE2: gadget_create(s); break;
-      case ZK_ES_ErrorOutOfGasSloadSstore: gadget_error_oog_sload_sstore(s); break;
-      case ZK_ES_ErrorOutOfGasCREATE: gadget_error_oog_create(s); break;
-      case ZK_ES_ErrorOutOfGasPrecompile: gadget_error_oog_precompile(s); break;
-      case ZK_ES_ErrorGasUintOverflow: gadget_error_gas_uint_overflow(s); break;
-      default: break;
-    }
-  } else if constexpr (G == KG_ARITH) {
-    switch (st) {
-      case ZK_ES_ADDMOD: gadget_addmod_mulmod(s, false); break;
-      case ZK_ES_MULMOD: gadget_addmod_mulmod(s, true); break;
-      case ZK_ES_SDIV_SMOD: gadget_sdiv_smod(s); break;
-      case ZK_ES_SAR: gadget_sar(s); break;
-      case ZK_ES_EXP: gadget_exp(s); break;
-      default: break;
-    }
+#define ZK_X(state, needs, call) \
+  case state: call; break;
+#define ZK_S(state, needs) case state:
+#define ZK_Y(group, list)              \
+  if constexpr (G == group) {          \
+    switch (st) {                      \
+      list(ZK_X, ZK_S) default: break; \
+    }                                  \
   }
+  ZK_EVM_GROUPS(ZK_Y)
+#undef ZK_Y
+#undef ZK_S
+#undef ZK_X
 }
 
 // whole step on one thread (tests/emu)
