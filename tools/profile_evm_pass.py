@@ -6,9 +6,11 @@ Runs the same upload and hot path as `bench.py` (invalidate every index, then on
 stream, under torch.profiler with CUDA activities.  A one-element torch kernel between passes marks the pass
 boundaries; it is left out of the listing.  Writes DIR/evm_pass_kernels.txt:
   - every device operation of one pass in the middle of the run: start (us from the pass's first operation),
-    duration, idle gap before it;
+    duration, gap from the latest end of the operations before it (negative: it overlaps them, as the hot kernels
+    on their own streams do);
   - per operation name: count per pass and mean duration over all profiled passes;
-  - index phase (everything before the first k_evm_classify), check phase (the rest) and the pass span.
+  - index phase (everything before the first k_evm_classify), check phase (the rest), hot phase (first start to
+    last end of k_evm_push_* and k_evm_gadget) and the pass span.
 """
 import argparse
 import json
@@ -83,12 +85,13 @@ def main():
     lines = [f"{args.passes} passes of {n} steps; library launches per pass {launches:.1f}", ""]
     mid = passes[len(passes) // 2]
     t0, prev_end = mid[0][1], mid[0][1]
-    lines.append(f"{'start_us':>9} {'dur_us':>8} {'gap_us':>7}  op")
+    lines.append(f"{'start_us':>9} {'dur_us':>8} {'gap_us':>7}  op (gap < 0: overlap)")
     for name, ts, dur in mid:
         lines.append(f"{ts - t0:9.1f} {dur:8.1f} {ts - prev_end:7.1f}  {name}")
         prev_end = max(prev_end, ts + dur)
     stats = {}
-    idx_ms, chk_ms, span_ms = [], [], []
+    idx_ms, chk_ms, hot_ms, span_ms = [], [], [], []
+    is_hot = lambda name: name.startswith(("k_evm_push", "k_evm_gadget"))  # noqa: E731
     for p in passes:
         seen = {}
         for name, ts, dur in p:
@@ -101,6 +104,9 @@ def main():
         cls = next((ts for name, ts, _ in p if name.startswith("k_evm_classify")), end)
         idx_ms.append((cls - start) / 1e3)
         chk_ms.append((end - cls) / 1e3)
+        hot = [(ts, ts + d) for name, ts, d in p if is_hot(name)]
+        if hot:
+            hot_ms.append((max(e for _, e in hot) - min(s for s, _ in hot)) / 1e3)
         span_ms.append((end - start) / 1e3)
     lines += ["", f"{'per_pass':>8} {'mean_us':>8}  op"]
     for name, (c, tot) in sorted(stats.items(), key=lambda kv: -kv[1][1]):
@@ -108,6 +114,7 @@ def main():
     mean = lambda xs: sum(xs) / len(xs)  # noqa: E731
     lines += ["", f"index phase (first op -> k_evm_classify start): {mean(idx_ms):.4f} ms",
               f"check phase (k_evm_classify start -> last op end): {mean(chk_ms):.4f} ms",
+              f"hot phase (first hot kernel start -> last hot kernel end): {mean(hot_ms) if hot_ms else 0:.4f} ms",
               f"pass span: {mean(span_ms):.4f} ms over {len(passes)} passes"]
     with open(os.path.join(args.out, "evm_pass_kernels.txt"), "w") as f:
         f.write("\n".join(lines) + "\n")

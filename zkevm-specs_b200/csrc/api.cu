@@ -117,7 +117,7 @@ struct zk_ctx {
   u64 resp_bitmap_version = ~0ull;
   unsigned char* stage = nullptr;  // device staging (zk_upload_bytecode_table_from_code)
   size_t stage_cap = 0;
-  unsigned char* evm_sort = nullptr;  // EvmSort arrays: bucket[cap] | sorted[cap] | hist, cursor, done, offs
+  unsigned char* evm_sort = nullptr;  // EvmSort arrays: bucket[cap] | sorted[cap] | hist, cursor, done, next_chunk, offs
   size_t evm_sort_cap = 0;
   u32* evm_hist_host = nullptr;  // pinned, mapped: histogram + positional flag, written by k_evm_classify's last block
   u32* evm_hist_mapped = nullptr;  // its device address
@@ -126,6 +126,10 @@ struct zk_ctx {
   // own stream next to the hot kernels; forked after the scatter, joined before the check returns to the caller's stream
   cudaStream_t evm_aux = nullptr;
   cudaEvent_t evm_fork_ev = nullptr, evm_join_ev = nullptr;
+  // the MUL, ADD and POP kernels run on streams of their own next to PUSH's (on the caller's stream): the blocks of one
+  // hot kernel take the SMs the others' retired blocks leave; each joins the caller's stream before the rare groups
+  cudaStream_t evm_hot[3] = {nullptr, nullptr, nullptr};
+  cudaEvent_t evm_hot_join[3] = {nullptr, nullptr, nullptr};
   int evm_tx_overlap = 1;  // env ZKCHECK_TX_OVERLAP at context creation ("0..." = in-line order)
   std::unordered_map<const void*, int> occ;  // resident blocks per SM of each kernel launched with a persistent grid
   BlockStats* block_stats = nullptr;  // k_evm_block_stats output
@@ -240,6 +244,10 @@ extern "C" void zk_ctx_destroy(zk_ctx* ctx) {
   if (ctx->evm_fork_ev) cudaEventDestroy(ctx->evm_fork_ev);
   if (ctx->evm_join_ev) cudaEventDestroy(ctx->evm_join_ev);
   if (ctx->evm_aux) cudaStreamDestroy(ctx->evm_aux);
+  for (int j = 0; j < 3; j++) {
+    if (ctx->evm_hot_join[j]) cudaEventDestroy(ctx->evm_hot_join[j]);
+    if (ctx->evm_hot[j]) cudaStreamDestroy(ctx->evm_hot[j]);
+  }
   if (ctx->resp_bitmap) cudaFree(ctx->resp_bitmap);
   delete ctx;
 }
@@ -1237,7 +1245,7 @@ static int check_evm(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStrea
   if (n > ctx->evm_sort_cap) {
     if (ctx->evm_sort) cudaFree(ctx->evm_sort);
     ctx->evm_sort = nullptr;
-    CK(ctx, cudaMalloc(&ctx->evm_sort, up256(n) + up256(n * 4) + (3 * ZK_EVM_NB + 3) * sizeof(u32)));
+    CK(ctx, cudaMalloc(&ctx->evm_sort, up256(n) + up256(n * 4) + (3 * ZK_EVM_NB + 3 + KG_COUNT) * sizeof(u32)));
     ctx->evm_sort_cap = n;
   }
   if (!ctx->evm_hist_host) {
@@ -1251,9 +1259,10 @@ static int check_evm(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStrea
   so.hist = (u32*)(ctx->evm_sort + up256(ctx->evm_sort_cap) + up256(ctx->evm_sort_cap * 4));
   so.cursor = so.hist + ZK_EVM_NB + 1;
   so.done = so.cursor + ZK_EVM_NB;
-  so.offs = so.done + 1;
+  so.next_chunk = so.done + 1;
+  so.offs = so.next_chunk + KG_COUNT;
   so.host_hist = ctx->evm_hist_mapped;
-  CK(ctx, cudaMemsetAsync(so.hist, 0, (2 * ZK_EVM_NB + 2) * sizeof(u32), st));
+  CK(ctx, cudaMemsetAsync(so.hist, 0, (2 * ZK_EVM_NB + 2 + KG_COUNT) * sizeof(u32), st));  // hist .. next_chunk
   const WitnessDev wd = witness_dev(m);
   const unsigned sort_grid = (unsigned)((n + 1023) / 1024);
   // the narrow instance needs 40 registers: blocks of ZK_CLASSIFY_THREADS = 512 keep 48 warps resident per SM instead of 32
@@ -1294,7 +1303,8 @@ static int check_evm(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStrea
     if ((rc = launched(ctx, "k_evm_block_stats"))) return rc;
     t.stats = ctx->block_stats;
   }
-  // one kernel per non-empty group, on a persistent grid: each thread walks its buckets with a grid stride
+  // one kernel per non-empty group, on a persistent grid: the hot groups' warps take chunks of their work queue, the
+  // rare groups' threads walk their buckets with a grid stride
   using EvmKernel = void (*)(WitnessDev, CheckRange, EvmTables, ResultDev, EvmSort);
   auto launch = [&](int g, EvmKernel kernel, const char* name, u64 threads_per_step, cudaStream_t s) {
     if (!group_n[g]) return 0;
@@ -1311,23 +1321,35 @@ static int check_evm(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStrea
   static const EvmKernel k_pop[3] = {k_evm_gadget<KG_POP, 0>, k_evm_gadget<KG_POP, 1>, k_evm_gadget<KG_POP, 2>};
   // the transaction-level group first, on the auxiliary stream: its blocks take their places before the hot kernels'
   // persistent grids fill the device, and its long per-thread chains run underneath them
+  if (!ctx->evm_fork_ev) CK(ctx, cudaEventCreateWithFlags(&ctx->evm_fork_ev, cudaEventDisableTiming));
+  CK(ctx, cudaEventRecord(ctx->evm_fork_ev, st));  // the sort and the on-demand indexes are done
   const bool tx_forked = group_n[KG_TX] && ctx->evm_tx_overlap;
   if (tx_forked) {
     if (!ctx->evm_aux) {
       CK(ctx, cudaStreamCreateWithFlags(&ctx->evm_aux, cudaStreamNonBlocking));
-      CK(ctx, cudaEventCreateWithFlags(&ctx->evm_fork_ev, cudaEventDisableTiming));
       CK(ctx, cudaEventCreateWithFlags(&ctx->evm_join_ev, cudaEventDisableTiming));
     }
-    CK(ctx, cudaEventRecord(ctx->evm_fork_ev, st));
     CK(ctx, cudaStreamWaitEvent(ctx->evm_aux, ctx->evm_fork_ev, 0));
     if ((rc = launch(KG_TX, k_evm_group<KG_TX>, "k_evm_group<KG_TX>", 1, ctx->evm_aux))) return rc;
     CK(ctx, cudaEventRecord(ctx->evm_join_ev, ctx->evm_aux));
   }
-  // k_evm_push_hash takes half a warp per step
-  if ((rc = launch(KG_PUSH, k_push[inst], inst ? "k_evm_push_pos" : "k_evm_push_hash", inst ? 1 : 16, st))) return rc;
-  if ((rc = launch(KG_MUL, k_mul[inst], "k_evm_gadget<KG_MUL>", 1, st))) return rc;
-  if ((rc = launch(KG_ADD, k_add[inst], "k_evm_gadget<KG_ADD>", 1, st))) return rc;
-  if ((rc = launch(KG_POP, k_pop[inst], "k_evm_gadget<KG_POP>", 1, st))) return rc;
+  // the hot kernels side by side: PUSH on the caller's stream, MUL, ADD and POP on streams of their own; a warp of
+  // k_evm_push_hash takes 32 steps per chunk like the others
+  if ((rc = launch(KG_PUSH, k_push[inst], inst ? "k_evm_push_pos" : "k_evm_push_hash", 1, st))) return rc;
+  const int hot_g[3] = {KG_MUL, KG_ADD, KG_POP};
+  const EvmKernel hot_k[3] = {k_mul[inst], k_add[inst], k_pop[inst]};
+  static const char* const hot_name[3] = {"k_evm_gadget<KG_MUL>", "k_evm_gadget<KG_ADD>", "k_evm_gadget<KG_POP>"};
+  for (int j = 0; j < 3; j++) {
+    if (!group_n[hot_g[j]]) continue;
+    if (!ctx->evm_hot[j]) {
+      CK(ctx, cudaStreamCreateWithFlags(&ctx->evm_hot[j], cudaStreamNonBlocking));
+      CK(ctx, cudaEventCreateWithFlags(&ctx->evm_hot_join[j], cudaEventDisableTiming));
+    }
+    CK(ctx, cudaStreamWaitEvent(ctx->evm_hot[j], ctx->evm_fork_ev, 0));
+    if ((rc = launch(hot_g[j], hot_k[j], hot_name[j], 1, ctx->evm_hot[j]))) return rc;
+    CK(ctx, cudaEventRecord(ctx->evm_hot_join[j], ctx->evm_hot[j]));
+    CK(ctx, cudaStreamWaitEvent(st, ctx->evm_hot_join[j], 0));
+  }
   if ((rc = launch(KG_SIMPLE, k_evm_group<KG_SIMPLE>, "k_evm_group<KG_SIMPLE>", 1, st))) return rc;
   if ((rc = launch(KG_BYTES32, k_evm_group<KG_BYTES32>, "k_evm_group<KG_BYTES32>", 1, st))) return rc;
   if ((rc = launch(KG_COPY, k_evm_group<KG_COPY>, "k_evm_group<KG_COPY>", 1, st))) return rc;

@@ -1900,6 +1900,7 @@ struct EvmSort {
   u32* hist;              // [ZK_EVM_NB + 1] steps per bucket; entry ZK_EVM_NB: 1 iff rw + bytecode tables are positional
   u32* cursor;            // [ZK_EVM_NB] scatter cursors (zeroed by the host)
   u32* done;              // [1] k_evm_classify blocks finished (zeroed by the host)
+  u32* next_chunk;        // [KG_COUNT] work queue of each hot group: chunks of 32 sorted entries taken (zeroed by the host)
   u32* offs;              // [ZK_EVM_NB + 1] first entry of each bucket in `sorted`
   u32* sorted;            // [n] local step indices, bucket by bucket
   u32* host_hist;         // [ZK_EVM_NB + 1] mapped pinned host memory: `hist` as k_evm_classify's last block leaves it
@@ -2049,33 +2050,25 @@ __global__ void __launch_bounds__(1024) k_evm_scatter(EvmSort so, u32 n) {
   if (blockIdx.x == 0 && threadIdx.x <= ZK_EVM_NB) so.offs[threadIdx.x] = s_off[threadIdx.x];
 }
 
+// Work queue of the hot kernels (k_evm_gadget, k_evm_push_*): a group's buckets are cut into chunks of 32
+// consecutive sorted entries, numbered bucket after bucket, and a warp runs one chunk at a time, so its lanes stay
+// on one gate program.  A grid-stride walk would make every thread run as many rounds as the busiest one, each a
+// full dependent chain of loads, even when the last round holds a few steps; with the queue, warps that run out of
+// chunks retire and their SMs take the next hot kernel's blocks.  Warp w takes chunk w first (no atomic: a grid
+// sized for the device has its whole first round resident), then one chunk per atomicAdd of lane 0 on the group's
+// counter (EvmSort::next_chunk), broadcast to the warp.  Every lane of the block is present (blocks of 128 threads).
+__device__ __forceinline__ u32 warp_first_chunk() { return (blockIdx.x * blockDim.x + threadIdx.x) >> 5; }
+__device__ __forceinline__ u32 warp_next_chunk(u32* counter) {
+  u32 c = 0;
+  if ((threadIdx.x & 31) == 0) c = atomicAdd(counter, 1u);
+  return ((gridDim.x * blockDim.x) >> 5) + __shfl_sync(0xFFFFFFFFu, c, 0);
+}
+
 // one thread per step for the gadgets whose work is a handful of independent lookups.
 // POS = both tables positional (known to the host from the read-back flag): that instance is compiled
 // with pos_mode = 1, i.e. without any hash-index code — these kernels were stalling on instruction
 // fetch ("no instruction" stalls), the executed path is now half as long.
 // POS: 0 = hash indexes, 1 = both tables positional, 2 = positional AND narrow (StepCtx::narrow)
-template <int G, int POS>
-__device__ __forceinline__ void bucket_steps(const WitnessDev& w, const CheckRange& rg, const EvmTables& t,
-                                             const ResultDev& res, const EvmSort& so, const u32* s_resp, int bucket,
-                                             const Fr* stack_pre, const u64& rw_base) {
-  // every lane of a warp runs the same number of rounds and calls the (warp-synchronous) lookups
-  // together; lanes without a step in the last round run with live = false
-  const u32 n = so.hist[bucket];
-  if (n == 0) return;
-  const u32* list = so.sorted + so.offs[bucket];
-  const u32 stride = gridDim.x * blockDim.x;
-  const u32 tid = blockIdx.x * blockDim.x + threadIdx.x;
-  for (u32 first = 0; first < n; first += stride) {
-    const u32 k = first + tid;
-    const bool live = k < n;
-    const u64 i = rg.row_begin + list[live ? k : 0];
-    StepCtx s{w, t, res, i, i + 1, rg.row_base + i, live, s_resp, 0xFFFFFFFFu, POS ? nullptr : stack_pre,
-              POS ? &rw_base : nullptr, POS ? 1 : -1, POS == 2 ? 1 : 0};
-    if (G == KG_ADD) gadget_add(s, live);
-    else if (G == KG_MUL) gadget_mul(s, live);
-    else gadget_pop(s, live);
-  }
-}
 // minimum resident blocks per SM (= register caps of 168 / 128); override with -D to sweep them
 #ifndef ZK_GADGET_MINBLOCKS
 #define ZK_GADGET_MINBLOCKS 3
@@ -2101,12 +2094,28 @@ k_evm_gadget(const __grid_constant__ WitnessDev w, const __grid_constant__ Check
   Fr stack_pre[2];
   if (!POS) stack_key_pre(t.rw, stack_pre);
   const u64 rw_base = POS ? table_cell(t.rw.tab, 0, 0).l[0] : 0;
-  if (G == KG_MUL) {  // three buckets (opcode peeks MUL / DIV / MOD), one after the other: warps stay uniform
-#pragma unroll 1
-    for (int sub = 0; sub < 3; sub++)
-      bucket_steps<G, POS>(w, rg, t, res, so, s_resp, sub == 0 ? ZK_ES_MUL : (sub == 1 ? ZK_BK_DIV : ZK_BK_MOD), stack_pre, rw_base);
-  } else {
-    bucket_steps<G, POS>(w, rg, t, res, so, s_resp, G == KG_ADD ? ZK_ES_ADD : ZK_ES_POP, stack_pre, rw_base);
+  // one chunk space: MUL's chunks are those of its MUL, DIV and MOD buckets (the opcode peeks), in that order
+  const u32 n0 = so.hist[G == KG_MUL ? ZK_ES_MUL : (G == KG_ADD ? ZK_ES_ADD : ZK_ES_POP)];
+  const u32 n1 = G == KG_MUL ? so.hist[ZK_BK_DIV] : 0, n2 = G == KG_MUL ? so.hist[ZK_BK_MOD] : 0;
+  const u32 c1 = (n0 + 31) / 32, c2 = c1 + (n1 + 31) / 32, n_chunks = c2 + (n2 + 31) / 32;
+  const unsigned lane = threadIdx.x & 31;
+  for (u32 c = warp_first_chunk(); c < n_chunks; c = warp_next_chunk(&so.next_chunk[G])) {
+    // every lane of a warp calls the (warp-synchronous) lookups together; lanes past the end of a bucket's last chunk
+    // run with live = false
+    u32 k = (c << 5) + lane, n = n0, off = so.offs[G == KG_MUL ? ZK_ES_MUL : (G == KG_ADD ? ZK_ES_ADD : ZK_ES_POP)];
+    if (G == KG_MUL && c >= c1) {
+      const bool mod = c >= c2;
+      k = ((c - (mod ? c2 : c1)) << 5) + lane;
+      n = mod ? n2 : n1;
+      off = so.offs[mod ? ZK_BK_MOD : ZK_BK_DIV];
+    }
+    const bool live = k < n;
+    const u64 i = rg.row_begin + so.sorted[off + (live ? k : 0)];
+    StepCtx s{w, t, res, i, i + 1, rg.row_base + i, live, s_resp, 0xFFFFFFFFu, POS ? nullptr : stack_pre,
+              POS ? &rw_base : nullptr, POS ? 1 : -1, POS == 2 ? 1 : 0};
+    if (G == KG_ADD) gadget_add(s, live);
+    else if (G == KG_MUL) gadget_mul(s, live);
+    else gadget_pop(s, live);
   }
 }
 
@@ -2160,11 +2169,14 @@ __global__ void __launch_bounds__(128, ZK_PUSH_MINBLOCKS) k_evm_push_pos(const _
   HeadCache hc{};
   const u32 n = so.hist[ZK_ES_PUSH];
   const u32* list = so.sorted + so.offs[ZK_ES_PUSH];
-  const u32 stride = gridDim.x * blockDim.x;
-  for (u32 k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += stride) {
-    const u64 i = rg.row_begin + list[k];
-    StepCtx s{w, t, res, i, i + 1, rg.row_base + i, true, s_resp, 1u << (threadIdx.x & 31), nullptr, &rw_base, 1, NARROW};
-    gadget_push_pos1(s, &hc);
+  const u32 n_chunks = (n + 31) / 32;
+  for (u32 c = warp_first_chunk(); c < n_chunks; c = warp_next_chunk(&so.next_chunk[KG_PUSH])) {
+    const u32 k = (c << 5) + (threadIdx.x & 31);
+    if (k < n) {  // the lookups here are lane-private
+      const u64 i = rg.row_begin + list[k];
+      StepCtx s{w, t, res, i, i + 1, rg.row_base + i, true, s_resp, 1u << (threadIdx.x & 31), nullptr, &rw_base, 1, NARROW};
+      gadget_push_pos1(s, &hc);
+    }
   }
 }
 
@@ -2174,7 +2186,7 @@ __global__ void __launch_bounds__(128, ZK_PUSH_MINBLOCKS) k_evm_push_pos(const _
 // the warp-instructions per step and doubles the steps in flight per warp; the kernel is
 // latency-bound on ~8 dependent memory round trips per step.  All 32 lanes
 // call every warp-synchronous lookup together; a half without a step (odd count) or whose step
-// already failed passes live = false.
+// already failed passes live = false.  A warp's chunk of the work queue (32 steps) is 16 such iterations.
 __global__ void __launch_bounds__(128, 4) k_evm_push_hash(const __grid_constant__ WitnessDev w, const __grid_constant__ CheckRange rg, const __grid_constant__ EvmTables t, const __grid_constant__ ResultDev res,
                 const __grid_constant__ EvmSort so) {
   __shared__ alignas(16) u32 s_resp[ZK_RESP_BITMAP_WORDS];
@@ -2187,10 +2199,10 @@ __global__ void __launch_bounds__(128, 4) k_evm_push_hash(const __grid_constant_
   const u32 n = so.hist[ZK_ES_PUSH];
   const u32* list = so.sorted + so.offs[ZK_ES_PUSH];
   const int lane = threadIdx.x & 31, half = lane >> 4, sub = lane & 15;
-  const u32 warps = (gridDim.x * blockDim.x) >> 5;
   const u32 n_pairs = (n + 1) >> 1;
   const int kNone = 0x7FFFFFFF;
-  for (u32 kp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; kp < n_pairs; kp += warps) {  // warp-uniform
+  for (u32 c = warp_first_chunk(); c < (n + 31) / 32; c = warp_next_chunk(&so.next_chunk[KG_PUSH]))
+  for (u32 kp = c * 16; kp < min(c * 16 + 16, n_pairs); kp++) {
     const u32 k = 2 * kp + half;
     const bool have = k < n;
     bool live = have;
