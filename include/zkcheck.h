@@ -143,7 +143,12 @@ int zk_set_challenge(zk_ctx* ctx, int which, const uint64_t r[4]);
 int zk_upload_columns(zk_ctx* ctx, int circuit_id, uint64_t n_rows, uint32_t n_cols,
                       const uint64_t* colmajor, void* stream);
 /* Same, but the matrix already lives in device memory (e.g. a torch tensor); the context
- * borrows the pointer until the next upload/bind for this circuit. */
+ * borrows the pointer until the next upload/bind for this circuit.  The kernels read it in
+ * place with 16-byte loads, so the pointer must be 16-byte aligned and must be device (or
+ * managed) memory of the context's device; NULL is allowed only with n_rows == 0.  Any
+ * other pointer returns -1 and leaves the previous matrix in place.  Binding the same
+ * pointer again after changing its contents counts as new contents (indexes are rebuilt).
+ * The same rules hold for zk_bind_table_device. */
 int zk_bind_columns_device(zk_ctx* ctx, int circuit_id, uint64_t n_rows, uint32_t n_cols,
                            const uint64_t* colmajor_device);
 

@@ -361,6 +361,9 @@ extern "C" int emu_check_bytecode(const uint64_t* cols, uint64_t n_rows, const u
   IndexStore s1, s2;
   IndexDev push_ix = build_index((const u64*)push, n_push, 2, pk, 2, ch, s1);
   IndexDev kec_ix = build_index((const u64*)keccak, n_keccak, 5, kk, 5, ch, s2);
+  PosState p_push;  // api.cu check_bytecode: the push table is served by position when it is dense from its first row
+  if (g_emu_positional) add_positional(push_ix, ZK_POS_DENSE, p_push);
+  g_emu_pos_ok = pos_enabled(push_ix) ? 1 : 0;
   Store ws;
   WitnessDev w = make_witness(ws, (const u64*)cols, n_rows, 12, nullptr);
   CheckRange rg{row_begin, row_end, 0, flags};

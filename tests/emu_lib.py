@@ -128,7 +128,8 @@ def set_positional(on: bool) -> None:
 
 
 def positional_tables() -> int:
-    """which tables of the last EVM / copy check took the positional lookup path: bit 0 bytecode, bit 1 rw"""
+    """which tables of the last EVM / copy check took the positional lookup path: bit 0 bytecode, bit 1 rw; of the last
+    bytecode-circuit check: bit 0 the push table"""
     return ctypes.c_int.in_dll(lib(), "g_emu_pos_ok").value
 
 

@@ -97,6 +97,20 @@ def check_evm(steps, bytecode, rw, fixed, row_begin=0, row_end=None, row_base=0,
     return ff, fc
 
 
+def diff(ff, off):
+    """the constraint ids where a first_fail array differs from the oracle's, with both values"""
+    bad = np.nonzero(ff != off)[0]
+    return f"ids {bad[:8].tolist()} cuda {ff[bad][:8].tolist()} oracle {off[bad][:8].tolist()}"
+
+
+def same(got, want, what):
+    """assert (first_fail, fail_count) == the oracle's, array for array"""
+    ff, fc = got
+    off, ofc = want
+    assert np.array_equal(ff, off) and np.array_equal(fc, ofc), \
+        f"{what}: {diff(ff, off)}; counts differ at {np.nonzero(fc != ofc)[0][:8].tolist()}"
+
+
 def constraint_classes(circuit_id):
     L = lib()
     n = L.orc_n_constraints(circuit_id)

@@ -11,10 +11,14 @@ from zkevm_specs_b200.evm_circuit.table import fixed_table_matrix
 
 
 def test_emu_bytecode_equals_oracle_on_goldens():
+    """both push-table paths: positional (the regular table, verified on the fly) and hash index only"""
     for name, k, cols, push, kec, r, exp_row, exp_exc in golden_util.bytecode_vectors():
-        ff, fc = emu_lib.check_bytecode(cols, push, kec, r)
         off, ofc = oracle_lib.check_bytecode(cols, push, kec, r)
-        assert np.array_equal(ff, off) and np.array_equal(fc, ofc), f"{name}[{k}]"
+        for positional in (True, False):
+            emu_lib.set_positional(positional)
+            ff, fc = emu_lib.check_bytecode(cols, push, kec, r)
+            assert np.array_equal(ff, off) and np.array_equal(fc, ofc), f"{name}[{k}] positional={positional}"
+    emu_lib.set_positional(True)
 
 
 def test_emu_evm_equals_oracle_on_goldens():

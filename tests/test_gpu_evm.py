@@ -278,9 +278,7 @@ def memory_family_vectors():
     return itertools.chain(golden_util.evm4_vectors(), golden_util.evm5_vectors(), golden_util.evm6_vectors(), golden_util.evm7_vectors(), golden_util.evm8_vectors(), golden_util.evm9_vectors(), golden_util.evm10_vectors(), golden_util.evm12_vectors(), golden_util.evm13_vectors(), golden_util.evm14_vectors(), golden_util.evm15_vectors(), golden_util.evm16_vectors(), golden_util.evm17_vectors(), golden_util.evm18_vectors(), golden_util.evm19_vectors(), golden_util.evm20_vectors(), golden_util.evm21_vectors(), golden_util.evm22_vectors(), golden_util.evm23_vectors(), golden_util.evm24_vectors(), golden_util.evm25_vectors(), golden_util.evm26_vectors(), golden_util.evm27_vectors(), golden_util.evm28_vectors())
 
 
-def _diff(ff, off):
-    bad = np.nonzero(ff != off)[0]
-    return f"ids {bad[:8].tolist()} cuda {ff[bad][:8].tolist()} oracle {off[bad][:8].tolist()}"
+_diff = oracle_lib.diff
 
 
 def test_evm_begin_end_tx_end_block_golden_and_oracle_parity():

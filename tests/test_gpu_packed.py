@@ -26,6 +26,7 @@ def test_every_golden_family_with_packed_storage(packed_ctx):
     import test_gpu_copy
     import test_gpu_evm
     import test_gpu_exp
+    import test_gpu_pi
     import test_gpu_state
 
     before = packed_ctx.launch_count()
@@ -40,6 +41,7 @@ def test_every_golden_family_with_packed_storage(packed_ctx):
     test_gpu_state.test_state_golden_and_oracle_parity()
     test_gpu_state.test_state_sharded_rows_match_whole()
     test_gpu_exp.test_exp_golden_and_oracle_parity()
+    test_gpu_pi.test_pi_golden_and_oracle_parity()
     assert packed_ctx.launch_count() > before
 
 

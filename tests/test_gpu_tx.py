@@ -97,30 +97,42 @@ def test_sig_golden_and_oracle_parity():
     assert n > 700
 
 
-def test_sig_verify_circuit_host_api_and_scale():
-    """host API like tests/test_sig_circuit.py; then 2^14 rows in one check (64 Fr products per row)"""
+class _LE:
+    def __init__(self, v):
+        self.le_bytes = int(v).to_bytes(32, "little")
+
+
+class _SigChip:
+    """stands in for the ECDSA chip of the sig circuit (sig_circuit.py): its verdict is given"""
+
+    def __init__(self, pk, msg, ok=True):
+        self.pub_key_x_bytes, self.pub_key_y_bytes = bytes(reversed(pk[:32])), bytes(reversed(pk[32:]))
+        self.msg_hash_bytes, self.sig_v, self.sig_r, self.sig_s, self.ok = msg, _LE(1), _LE(12345), _LE(67890), ok
+
+    def verify(self):
+        return self.ok
+
+
+def _sig_rows(r):
+    """six signatures, the one at row 4 invalid (and marked so): (rows, keccak table) of a valid sig witness"""
     from zkevm_specs_b200 import sig_circuit as sc
 
-    class LE:
-        def __init__(self, v):
-            self.le_bytes = int(v).to_bytes(32, "little")
-
-    class Chip:
-        def __init__(self, pk, msg, ok=True):
-            self.pub_key_x_bytes, self.pub_key_y_bytes = bytes(reversed(pk[:32])), bytes(reversed(pk[32:]))
-            self.msg_hash_bytes, self.sig_v, self.sig_r, self.sig_s, self.ok = msg, LE(1), LE(12345), LE(67890), ok
-
-        def verify(self):
-            return self.ok
-
-    r = FQ(0x77777777777777777)
     rng = np.random.default_rng(9)
     kt, rows = tc.KeccakTable(), []
     for i in range(6):
         pk, msg = bytes(rng.integers(0, 256, 64, dtype=np.uint8)), bytes(rng.integers(0, 256, 32, dtype=np.uint8))
         kt.add(pk, r)
         h = keccak256(pk)
-        rows.append(sc.Row(h, FQ(int.from_bytes(h[-20:], "big")), Word(msg), Chip(pk, msg, ok=i != 4), is_valid=i != 4))
+        rows.append(sc.Row(h, FQ(int.from_bytes(h[-20:], "big")), Word(msg), _SigChip(pk, msg, ok=i != 4), is_valid=i != 4))
+    return rows, kt
+
+
+def test_sig_verify_circuit_host_api_and_scale():
+    """host API like tests/test_sig_circuit.py; then 2^14 rows in one check (64 Fr products per row)"""
+    from zkevm_specs_b200 import sig_circuit as sc
+
+    r = FQ(0x77777777777777777)
+    rows, kt = _sig_rows(r)
     sc.verify_circuit(sc.Witness(rows, kt), r)
     rows[2].recovered_addr = FQ(rows[2].recovered_addr.n ^ 1)
     with pytest.raises(AssertionError, match="row = 2"):

@@ -356,11 +356,32 @@ extern "C" int zk_upload_columns(zk_ctx* ctx, int circuit_id, uint64_t n_rows, u
   return store_matrix(ctx, ctx->circ[circuit_id], n_rows, n_cols, (const u64*)colmajor, nullptr,
                       (cudaStream_t)stream);
 }
+// A borrowed matrix is read in place by the kernels: cells with 16-byte vector loads (fr.cuh ld_cell) and the push
+// table with one bulk copy into shared memory (circuit.cuh stage_to_smem), so its base must be 16-byte aligned, and it
+// must be device (or managed) memory of the context's device.  Checked before anything is stored: a rejected bind
+// leaves the previous matrix in place.
+static int check_borrowed(zk_ctx* ctx, const void* dev, u64 n_rows) {
+  if (!dev) return n_rows ? fail_msg(ctx, "bound device pointer is null") : 0;
+  if ((uintptr_t)dev % 16) return fail_msg(ctx, "bound device pointer is not 16-byte aligned");
+  CK(ctx, cudaSetDevice(ctx->device));
+  cudaPointerAttributes a{};
+  const cudaError_t e = cudaPointerGetAttributes(&a, dev);
+  if (e != cudaSuccess) {
+    (void)cudaGetLastError();  // not a sticky error: clear it so the next launch check does not report it
+    return fail_msg(ctx, std::string("bound pointer is not device memory: ") + cudaGetErrorString(e));
+  }
+  if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged)
+    return fail_msg(ctx, "bound pointer is not device or managed memory");
+  if (a.device != ctx->device) return fail_msg(ctx, "bound pointer is memory of another device");
+  return 0;
+}
+
 extern "C" int zk_bind_columns_device(zk_ctx* ctx, int circuit_id, uint64_t n_rows, uint32_t n_cols,
                                       const uint64_t* dev) {
   if (circuit_id < 0 || circuit_id >= ZK_N_CIRCUITS) return fail_msg(ctx, "bad circuit id");
   if ((int)n_cols != kCircuitCols[circuit_id]) return fail_msg(ctx, "wrong column count for circuit");
   if (n_rows >= 0xFFFFFFFFull) return fail_msg(ctx, "too many rows (row ids are uint32)");
+  if (const int rc = check_borrowed(ctx, dev, n_rows)) return rc;
   return store_matrix(ctx, ctx->circ[circuit_id], n_rows, n_cols, nullptr, (const u64*)dev, 0);
 }
 extern "C" int zk_upload_row_flags(zk_ctx* ctx, int circuit_id, uint64_t n_rows,
@@ -381,6 +402,7 @@ extern "C" int zk_bind_table_device(zk_ctx* ctx, int table_id, uint64_t n_rows, 
   if (table_id < 0 || table_id >= ZK_N_TABLES) return fail_msg(ctx, "bad table id");
   if ((int)n_cols != kTableCols[table_id]) return fail_msg(ctx, "wrong column count for table");
   if (n_rows >= 0x7FFFFFFFull) return fail_msg(ctx, "too many table rows");
+  if (const int rc = check_borrowed(ctx, dev, n_rows)) return rc;
   return store_matrix(ctx, ctx->tab[table_id], n_rows, n_cols, nullptr, (const u64*)dev, 0);
 }
 extern "C" int zk_upload_table_flags(zk_ctx* ctx, int table_id, uint64_t n_rows,
