@@ -9,8 +9,9 @@ boundaries; it is left out of the listing.  Writes DIR/evm_pass_kernels.txt:
     duration, gap from the latest end of the operations before it (negative: it overlaps them, as the hot kernels
     on their own streams do);
   - per operation name: count per pass and mean duration over all profiled passes;
-  - index phase (everything before the first k_evm_classify), check phase (the rest), hot phase (first start to
-    last end of k_evm_push_* and k_evm_gadget) and the pass span.
+  - index phase (everything before k_evm_sort), check phase (the rest), the step sort (k_evm_sort's duration and
+    the gap from its start to the first hot kernel's start), hot phase (first start to last end of k_evm_push_* and
+    k_evm_gadget) and the pass span.
 """
 import argparse
 import json
@@ -90,7 +91,7 @@ def main():
         lines.append(f"{ts - t0:9.1f} {dur:8.1f} {ts - prev_end:7.1f}  {name}")
         prev_end = max(prev_end, ts + dur)
     stats = {}
-    idx_ms, chk_ms, hot_ms, span_ms = [], [], [], []
+    idx_ms, chk_ms, hot_ms, span_ms, sort_us, to_hot_us = [], [], [], [], [], []
     is_hot = lambda name: name.startswith(("k_evm_push", "k_evm_gadget"))  # noqa: E731
     for p in passes:
         seen = {}
@@ -101,19 +102,23 @@ def main():
             seen[name] = 1
         start = p[0][1]
         end = max(ts + d for _, ts, d in p)
-        cls = next((ts for name, ts, _ in p if name.startswith("k_evm_classify")), end)
-        idx_ms.append((cls - start) / 1e3)
-        chk_ms.append((end - cls) / 1e3)
+        srt = next(((ts, d) for name, ts, d in p if name.startswith("k_evm_sort")), (end, 0.0))
+        idx_ms.append((srt[0] - start) / 1e3)
+        chk_ms.append((end - srt[0]) / 1e3)
         hot = [(ts, ts + d) for name, ts, d in p if is_hot(name)]
         if hot:
             hot_ms.append((max(e for _, e in hot) - min(s for s, _ in hot)) / 1e3)
+            sort_us.append(srt[1])
+            to_hot_us.append(min(s for s, _ in hot) - srt[0])
         span_ms.append((end - start) / 1e3)
     lines += ["", f"{'per_pass':>8} {'mean_us':>8}  op"]
     for name, (c, tot) in sorted(stats.items(), key=lambda kv: -kv[1][1]):
         lines.append(f"{c / len(passes):8.2f} {tot / c:8.1f}  {name}")
     mean = lambda xs: sum(xs) / len(xs)  # noqa: E731
-    lines += ["", f"index phase (first op -> k_evm_classify start): {mean(idx_ms):.4f} ms",
-              f"check phase (k_evm_classify start -> last op end): {mean(chk_ms):.4f} ms",
+    lines += ["", f"index phase (first op -> k_evm_sort start): {mean(idx_ms):.4f} ms",
+              f"check phase (k_evm_sort start -> last op end): {mean(chk_ms):.4f} ms",
+              f"step sort: k_evm_sort {mean(sort_us) if sort_us else 0:.1f} us, its start -> first hot kernel start "
+              f"{mean(to_hot_us) if to_hot_us else 0:.1f} us",
               f"hot phase (first hot kernel start -> last hot kernel end): {mean(hot_ms) if hot_ms else 0:.4f} ms",
               f"pass span: {mean(span_ms):.4f} ms over {len(passes)} passes"]
     with open(os.path.join(args.out, "evm_pass_kernels.txt"), "w") as f:

@@ -9,6 +9,8 @@
 #include <string.h>
 
 #include <algorithm>
+#include <atomic>
+#include <chrono>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -117,13 +119,16 @@ struct zk_ctx {
   u64 resp_bitmap_version = ~0ull;
   unsigned char* stage = nullptr;  // device staging (zk_upload_bytecode_table_from_code)
   size_t stage_cap = 0;
-  unsigned char* evm_sort = nullptr;  // EvmSort arrays: bucket[cap] | sorted[cap] | hist, cursor, done, next_chunk, offs
+  unsigned char* evm_sort = nullptr;  // EvmSort arrays: bucket[cap] | sorted[cap] | hist, cursor, next_chunk, offs
   size_t evm_sort_cap = 0;
-  u32* evm_hist_host = nullptr;  // pinned, mapped: histogram + positional flag, written by k_evm_classify's last block
+  // pinned, mapped: histogram + positional flag, then the sequence number of the check that wrote them (k_evm_sort's
+  // block 0, right after its barrier)
+  u32* evm_hist_host = nullptr;
   u32* evm_hist_mapped = nullptr;  // its device address
-  cudaEvent_t evm_hist_ev = nullptr;
+  u32 evm_sort_seq = 0;            // sequence number of the latest check_evm of this context
+  cudaEvent_t evm_hist_ev = nullptr;  // recorded after k_evm_sort: bounds the host's wait for the histogram
   // the transaction-level group (k_evm_group<TX>: a few thousand threads, each a chain of dependent lookups) runs on its
-  // own stream next to the hot kernels; forked after the scatter, joined before the check returns to the caller's stream
+  // own stream next to the hot kernels; forked after the step sort, joined before the check returns to the caller's stream
   cudaStream_t evm_aux = nullptr;
   cudaEvent_t evm_fork_ev = nullptr, evm_join_ev = nullptr;
   // the MUL, ADD and POP kernels run on streams of their own next to PUSH's (on the caller's stream): the blocks of one
@@ -1261,17 +1266,17 @@ static int check_evm(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStrea
   t.wd = table_dev(ctx, ZK_TABLE_WITHDRAWAL);
   if ((rc = mark_indexes_ready(ctx))) return rc;
   const u64 n = rg.row_end - rg.row_begin;
-  // counting sort of the steps by execution state (k_evm_classify + k_evm_scatter), then one kernel
-  // per non-empty gate-program group
+  // counting sort of the steps by execution state (k_evm_sort), then one kernel per non-empty gate-program group
   auto up256 = [](size_t x) { return (x + 255) / 256 * 256; };
   if (n > ctx->evm_sort_cap) {
     if (ctx->evm_sort) cudaFree(ctx->evm_sort);
     ctx->evm_sort = nullptr;
-    CK(ctx, cudaMalloc(&ctx->evm_sort, up256(n) + up256(n * 4) + (3 * ZK_EVM_NB + 3 + KG_COUNT) * sizeof(u32)));
+    CK(ctx, cudaMalloc(&ctx->evm_sort, up256(n) + up256(n * 4) + (3 * ZK_EVM_NB + 2 + KG_COUNT) * sizeof(u32)));
     ctx->evm_sort_cap = n;
   }
   if (!ctx->evm_hist_host) {
-    CK(ctx, cudaHostAlloc(&ctx->evm_hist_host, (ZK_EVM_NB + 1) * sizeof(u32), cudaHostAllocMapped));
+    CK(ctx, cudaHostAlloc(&ctx->evm_hist_host, (ZK_EVM_NB + 2) * sizeof(u32), cudaHostAllocMapped));
+    memset(ctx->evm_hist_host, 0, (ZK_EVM_NB + 2) * sizeof(u32));  // no check has published yet (sequence numbers start at 1)
     CK(ctx, cudaHostGetDevicePointer((void**)&ctx->evm_hist_mapped, ctx->evm_hist_host, 0));
     CK(ctx, cudaEventCreateWithFlags(&ctx->evm_hist_ev, cudaEventDisableTiming));
   }
@@ -1280,27 +1285,45 @@ static int check_evm(zk_ctx* ctx, const CheckRange& rg, ResultDev res, cudaStrea
   so.sorted = (u32*)(ctx->evm_sort + up256(ctx->evm_sort_cap));
   so.hist = (u32*)(ctx->evm_sort + up256(ctx->evm_sort_cap) + up256(ctx->evm_sort_cap * 4));
   so.cursor = so.hist + ZK_EVM_NB + 1;
-  so.done = so.cursor + ZK_EVM_NB;
-  so.next_chunk = so.done + 1;
+  so.next_chunk = so.cursor + ZK_EVM_NB;
   so.offs = so.next_chunk + KG_COUNT;
   so.host_hist = ctx->evm_hist_mapped;
-  CK(ctx, cudaMemsetAsync(so.hist, 0, (2 * ZK_EVM_NB + 2 + KG_COUNT) * sizeof(u32), st));  // hist .. next_chunk
-  const WitnessDev wd = witness_dev(m);
-  const unsigned sort_grid = (unsigned)((n + 1023) / 1024);
-  // the narrow instance needs 40 registers: blocks of ZK_CLASSIFY_THREADS = 512 keep 48 warps resident per SM instead of 32
-#ifndef ZK_CLASSIFY_THREADS
-#define ZK_CLASSIFY_THREADS 512
+  CK(ctx, cudaMemsetAsync(so.hist, 0, (2 * ZK_EVM_NB + 1 + KG_COUNT) * sizeof(u32), st));  // hist .. next_chunk
+  WitnessDev wd = witness_dev(m);
+  if (++ctx->evm_sort_seq == 0) ctx->evm_sort_seq = 1;  // 0: the buffer's initial value
+  u32 seq = ctx->evm_sort_seq;
+  // one cooperative launch on a persistent grid (k_evm_sort: the grid-wide barrier needs every block resident)
+  const bool narrow = evm_narrow(ctx);
+  const void* sort_k = narrow ? (const void*)k_evm_sort<1> : (const void*)k_evm_sort<0>;
+  const u64 spt = narrow ? ZK_SORT_SPT(1) : ZK_SORT_SPT(0);
+  const unsigned sort_grid = narrow ? grid_persistent(ctx, k_evm_sort<1>, ZK_SORT_THREADS, (n + spt - 1) / spt)
+                                    : grid_persistent(ctx, k_evm_sort<0>, ZK_SORT_THREADS, (n + spt - 1) / spt);
+  void* sort_args[] = {(void*)&wd, (void*)&rg, (void*)&t, (void*)&res, (void*)&so, (void*)&seq};
+  (void)cudaLaunchCooperativeKernel(sort_k, dim3(sort_grid), dim3(ZK_SORT_THREADS), sort_args, 0, st);
+  if ((rc = launched(ctx, "k_evm_sort"))) return rc;
+  CK(ctx, cudaEventRecord(ctx->evm_hist_ev, st));
+  // the histogram decides which groups run and how large their grids are.  Block 0 of the sort publishes it with this
+  // check's sequence number right after the barrier, and the device keeps scattering while the host launches.  The
+  // wait ends with an error if the sort completes (or fails) without publishing.  The event is queried at most every
+  // ZK_SORT_QUERY_US: a driver call in progress when the number lands delays the launches by its own duration.
+#ifndef ZK_SORT_QUERY_US
+#define ZK_SORT_QUERY_US 50
 #endif
-  if (evm_narrow(ctx)) k_evm_classify<1><<<(unsigned)((n + ZK_CLASSIFY_THREADS - 1) / ZK_CLASSIFY_THREADS), ZK_CLASSIFY_THREADS, 0, st>>>(wd, rg, t, res, so);
-  else k_evm_classify<0><<<sort_grid, 1024, 0, st>>>(wd, rg, t, res, so);
-  if ((rc = launched(ctx, "k_evm_classify"))) return rc;
-  CK(ctx, cudaEventRecord(ctx->evm_hist_ev, st));  // the histogram is in host memory once k_evm_classify is complete
-  k_evm_scatter<<<sort_grid, 1024, 0, st>>>(so, (u32)n);
-  if ((rc = launched(ctx, "k_evm_scatter"))) return rc;
-  // the histogram decides which groups run and how large their grids are; the device keeps working on
-  // the scatter meanwhile
-  CK(ctx, cudaEventSynchronize(ctx->evm_hist_ev));
-  const u32* hist = ctx->evm_hist_host;
+  volatile const u32* pub = ctx->evm_hist_host;
+  auto next_query = std::chrono::steady_clock::now() + std::chrono::microseconds(ZK_SORT_QUERY_US);
+  while (pub[ZK_EVM_NB + 1] != seq) {
+    const auto now = std::chrono::steady_clock::now();
+    if (now < next_query) continue;
+    next_query = now + std::chrono::microseconds(ZK_SORT_QUERY_US);
+    const cudaError_t e = cudaEventQuery(ctx->evm_hist_ev);
+    if (e == cudaErrorNotReady) continue;
+    if (e == cudaSuccess && pub[ZK_EVM_NB + 1] == seq) break;
+    if (e != cudaSuccess) CK(ctx, e);
+    return fail_msg(ctx, "k_evm_sort completed without publishing its histogram");
+  }
+  std::atomic_thread_fence(std::memory_order_acquire);
+  u32 hist[ZK_EVM_NB + 1];
+  for (int b = 0; b <= ZK_EVM_NB; b++) hist[b] = pub[b];
   const bool pos = hist[ZK_EVM_NB] != 0;
   u64 group_n[KG_COUNT] = {0};
   unsigned needs = 0;  // es_needs of the states present

@@ -33,8 +33,8 @@ enum { R_RWC, R_RW, R_TAG, R_ID, R_ADDR, R_FIELD, R_KEY_LO, R_KEY_HI, R_VAL_LO, 
 
 // ---- gate programs --------------------------------------------------------------------------
 // One kernel per GROUP of gate programs with similar register needs; inside a group kernel every
-// execution state has its own bucket of steps, so warps run one gate program (k_evm_classify /
-// k_evm_scatter sort the steps by state).  The host launches a group only when one of its buckets is
+// execution state has its own bucket of steps, so warps run one gate program (k_evm_sort sorts the
+// steps by state).  The host launches a group only when one of its buckets is
 // non-empty (check_evm reads the histogram back).  ADD / MUL / PUSH / POP are the hot groups, each with
 // kernels of its own (k_evm_gadget, k_evm_push_*); the others run in k_evm_group<G>.
 enum { KG_ADD, KG_MUL, KG_PUSH, KG_POP, KG_SIMPLE, KG_BYTES32, KG_COPY, KG_WIDE, KG_TX, KG_ARITH, KG_COUNT };
@@ -388,14 +388,14 @@ ZK_HD int rw_lookup(const StepCtx& s, bool live, const Fr& rwc, u64 rw, u64 tag,
 
 // ---- prologue: verify_step before the gadget (main.py:47-63, instruction.py:189-204) --------
 // Steps are bucketed by execution state (one bucket per state; the MUL state is split three ways by an
-// opcode peek, see k_evm_classify) and each bucket is run by the kernel of its gate-program group.
+// opcode peek, see k_evm_sort) and each bucket is run by the kernel of its gate-program group.
 #define ZK_EVM_NB 128      // bucket ids: execution states 0..ZK_ES_COUNT-1, then
 #define ZK_BK_DIV ZK_ES_COUNT        // MUL-state steps whose opcode peeks as DIV
 #define ZK_BK_MOD (ZK_ES_COUNT + 1)  // ... as MOD (everything else stays in bucket ZK_ES_MUL)
 #define ZK_BK_NONE 0xFF              // the step already failed in the prologue
 // returns the execution state whose gate program must run for this step, or -1 if the step already failed
-ZK_HD int step_prologue(const StepCtx& s, u32 flags) {
-  const Fr cs = s.cur(S_STATE), ns = s.nxt(S_STATE);
+// (cs, ns: the state cells of the step and of the next one, loaded by the caller)
+ZK_HD int step_prologue(const StepCtx& s, u32 flags, const Fr& cs, const Fr& ns) {
   const bool is_first = (flags & ZK_FLAG_EVM_FIRST_STEP) && s.row == 0;
   const bool is_last = (flags & ZK_FLAG_EVM_LAST_STEP) && s.i == s.w.n_rows - 2;
   const bool cs_small = fr_fits64(cs) && cs.l[0] < ZK_ES_COUNT;
@@ -422,6 +422,7 @@ ZK_HD int step_prologue(const StepCtx& s, u32 flags) {
   step_fail(s, EV_UNSUPPORTED_STATE);
   return -1;
 }
+ZK_HD int step_prologue(const StepCtx& s, u32 flags) { return step_prologue(s, flags, s.cur(S_STATE), s.nxt(S_STATE)); }
 
 // opcode_lookup(True) at the start of every hot gadget (instruction.py:784-790)
 ZK_HD bool opcode_lookup(const StepCtx& s, bool live, Fr* opcode) {
@@ -1838,7 +1839,7 @@ __host__ __device__ constexpr int es_group(int st) {
     ZK_EVM_GROUPS(ZK_Y)
 #undef ZK_Y
 #undef ZK_X
-    case ZK_BK_DIV: case ZK_BK_MOD: return KG_MUL;  // buckets of MUL-state steps (k_evm_classify), not states
+    case ZK_BK_DIV: case ZK_BK_MOD: return KG_MUL;  // buckets of MUL-state steps (k_evm_sort), not states
     default: return -1;
   }
 }
@@ -1891,19 +1892,19 @@ ZK_HD void verify_step(const StepCtx& s, u32 flags) {
 // kernels
 // ======================================================================================
 // The reference dispatches one Python gadget per step (execution/__init__.py:86-171).  Here the steps
-// are SORTED by execution state first — k_evm_classify runs the cheap prologue of every step, writes
-// its bucket and a histogram; k_evm_scatter turns the histogram into bucket offsets and writes the
-// step indices bucket by bucket (a counting sort, one byte + one u32 per step) — and then one kernel
-// per gate-program group walks its buckets, so the lanes of a warp run the same straight-line program.
+// are SORTED by execution state first — k_evm_sort runs the cheap prologue of every step, writes its
+// bucket and a histogram, and after a grid-wide barrier turns the histogram into bucket offsets and
+// writes the step indices bucket by bucket (a counting sort, one byte + one u32 per step) — and then one
+// kernel per gate-program group walks its buckets, so the lanes of a warp run the same straight-line program.
 struct EvmSort {
   unsigned char* bucket;  // [n] bucket of local step k (ZK_BK_NONE: it failed in the prologue)
   u32* hist;              // [ZK_EVM_NB + 1] steps per bucket; entry ZK_EVM_NB: 1 iff rw + bytecode tables are positional
   u32* cursor;            // [ZK_EVM_NB] scatter cursors (zeroed by the host)
-  u32* done;              // [1] k_evm_classify blocks finished (zeroed by the host)
   u32* next_chunk;        // [KG_COUNT] work queue of each hot group: chunks of 32 sorted entries taken (zeroed by the host)
   u32* offs;              // [ZK_EVM_NB + 1] first entry of each bucket in `sorted`
   u32* sorted;            // [n] local step indices, bucket by bucket
-  u32* host_hist;         // [ZK_EVM_NB + 1] mapped pinned host memory: `hist` as k_evm_classify's last block leaves it
+  u32* host_hist;         // [ZK_EVM_NB + 2] mapped pinned host memory: `hist`, then the sequence number of the check
+                          // that published it
 };
 
 // Table-derived constants of EndBlock (end_block.py:68-105).  The reference's tables are Python sets, so a
@@ -1961,62 +1962,136 @@ __global__ void __launch_bounds__(256) k_evm_block_stats(EvmTables t, BlockStats
 // MUL, DIV and MOD take three different witness-assignment branches (mul_div_mod.py:23-41), and a warp
 // that holds all three runs them one after the other.  The peek only chooses the bucket — the gate
 // program looks the opcode up again and decides everything itself — so a wrong peek costs time, never
-// the verdict.
-__device__ __forceinline__ int mul_bucket_peek(const StepCtx& s, const Fr& hlo, const Fr& hhi, const Fr& pc) {
-  u32 head = 0, len = 0;
-  if (heads_probe(s.t.bytecode, hlo, hhi, &head, &len, s.mask, true) != 1) return ZK_ES_MUL;
-  if (!(fr_fits64(pc) && pc.l[0] < (u64)len)) return ZK_ES_MUL;
-  const Fr v = table_cell(s.t.bytecode.tab, B_VALUE, (u64)head + 1 + pc.l[0]);
+// the verdict.  The peek is the heads-index probe of the step's code hash (n_head, head, len), then the
+// opcode byte at `pc` of that run: mul_peek_row gives the byte's row (false: the peek stops at ZK_ES_MUL),
+// mul_peek_bucket the bucket from the byte.
+__device__ __forceinline__ bool mul_peek_row(int n_head, u32 head, u32 len, const Fr& pc, u64* row) {
+  *row = (u64)head + 1 + pc.l[0];
+  return n_head == 1 && fr_fits64(pc) && pc.l[0] < (u64)len;
+}
+__device__ __forceinline__ int mul_peek_bucket(const Fr& v) {
   return fr_eq_u64(v, 4) ? ZK_BK_DIV : (fr_eq_u64(v, 6) ? ZK_BK_MOD : ZK_ES_MUL);
 }
 
+// The step sort in ONE cooperative launch on a persistent grid (one grid-wide barrier between the phases):
+//   1. classify: a thread takes ZK_SORT_SPT steps of a tile at a time (a tile is ZK_SORT_THREADS * ZK_SORT_SPT
+//      consecutive steps, a block walks every gridDim.x-th tile) and loads all their cells before it runs the
+//      prologue of any, so the thread has that many steps' loads in flight.  The MUL peek probes the heads index
+//      once per warp, for the code hash of the leading lane's first MUL-state step; a lane whose steps carry another
+//      hash probes for itself.  Buckets go to so.bucket; the block's histogram is kept in shared memory and added to
+//      so.hist with one atomic per non-empty bucket.
+//   2. after the barrier, block 0 first writes the histogram and the positional flag to the host's mapped buffer,
+//      then (behind a system-scope fence) `seq`: the host launches the gate-program kernels as soon as it sees its
+//      own sequence number there, while the grid scatters.  Every block scans the histogram, takes its base in each
+//      bucket with one atomic per non-empty bucket (its phase-1 counts are its share), and walks its tiles again,
+//      writing the sorted step indices.
 // NARROW: StepCtx::narrow (the step cells but the code hash sit in columns of at most 8 bytes: one aligned load each)
+#ifndef ZK_SORT_THREADS
+#define ZK_SORT_THREADS 256
+#endif
+#define ZK_SORT_SPT(NARROW) ((NARROW) ? 4 : 2)
 template <int NARROW>
-__global__ void __launch_bounds__(1024) k_evm_classify(const __grid_constant__ WitnessDev w, const __grid_constant__ CheckRange rg, const __grid_constant__ EvmTables t, const __grid_constant__ ResultDev res, const __grid_constant__ EvmSort so) {
-  // histogram aggregated per BLOCK: lanes of a warp that share a bucket elect a leader (match_any),
-  // leaders add to a shared histogram, one global atomicAdd per (block, non-empty bucket)
+__global__ void __launch_bounds__(ZK_SORT_THREADS, 2) k_evm_sort(const __grid_constant__ WitnessDev w, const __grid_constant__ CheckRange rg, const __grid_constant__ EvmTables t, const __grid_constant__ ResultDev res, const __grid_constant__ EvmSort so, u32 seq) {
+  namespace cg = cooperative_groups;
+  cg::grid_group grid = cg::this_grid();
+  constexpr int SPT = ZK_SORT_SPT(NARROW);
+  constexpr u32 TILE = ZK_SORT_THREADS * SPT;
+  // this block's steps per bucket (phase 1), then the next free entry of each bucket in its share (phase 2)
   __shared__ u32 s_hist[ZK_EVM_NB];
+  __shared__ u32 s_off[ZK_EVM_NB + 1], s_wsum[ZK_EVM_NB / 32];
   if (threadIdx.x < ZK_EVM_NB) s_hist[threadIdx.x] = 0;
   __syncthreads();
-  const u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-  const u64 i = rg.row_begin + k;
-  const unsigned lane = threadIdx.x & 31;
+  const u64 n = rg.row_end - rg.row_begin;
+  const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const bool pos = both_positional(t);
-  int b = ZK_BK_NONE;
-  if (i < rg.row_end) {
-    StepCtx s{w, t, res, i, i + 1, rg.row_base + i, true, nullptr, 1u << lane, nullptr, nullptr, -1, NARROW};
-    // the peek's cells are fetched with the state cells (one memory round trip instead of two)
-    const Fr hlo = s.cur(S_HASH_LO), hhi = s.cur(S_HASH_HI), pc = s.cur(S_PC);
-    const int st = step_prologue(s, rg.flags);
-    if (st >= 0) b = (st == ZK_ES_MUL && pos) ? mul_bucket_peek(s, hlo, hhi, pc) : st;
-    so.bucket[k] = (unsigned char)b;
+  for (u64 base = (u64)blockIdx.x * TILE; base < n; base += (u64)gridDim.x * TILE) {
+    // a code hash is kept as its two 128-bit halves and whether both fit them (heads_probe finds no other hash)
+    Fr cs[SPT], ns[SPT], pc[SPT];
+    u64 h[SPT][4];
+    bool hfit[SPT];
+    int b[SPT];
+#pragma unroll
+    for (int q = 0; q < SPT; q++) {  // every cell of the thread's steps first (steps past the end load the last one)
+      const u64 i = rg.row_begin + min(base + (u64)q * ZK_SORT_THREADS + threadIdx.x, n - 1);
+      StepCtx s{w, t, res, i, i + 1, rg.row_base + i, true, nullptr, 1u << lane, nullptr, nullptr, -1, NARROW};
+      cs[q] = s.cur(S_STATE);
+      ns[q] = s.nxt(S_STATE);
+      const Fr hlo = s.cur(S_HASH_LO), hhi = s.cur(S_HASH_HI);
+      h[q][0] = hlo.l[0], h[q][1] = hlo.l[1], h[q][2] = hhi.l[0], h[q][3] = hhi.l[1];
+      hfit[q] = fr_fits128(hlo) && fr_fits128(hhi);
+      pc[q] = s.cur(S_PC);
+    }
+    unsigned need = 0;  // bit q: step q is a MUL-state step and gets the peek
+#pragma unroll
+    for (int q = 0; q < SPT; q++) {
+      const u64 k = base + (u64)q * ZK_SORT_THREADS + threadIdx.x, i = rg.row_begin + k;
+      b[q] = ZK_BK_NONE;
+      if (k < n) {
+        StepCtx s{w, t, res, i, i + 1, rg.row_base + i, true, nullptr, 1u << lane, nullptr, nullptr, -1, NARROW};
+        const int st = step_prologue(s, rg.flags, cs[q], ns[q]);
+        if (st >= 0) b[q] = st;
+        if (st == ZK_ES_MUL && pos) need |= 1u << q;
+      }
+    }
+    const unsigned lanes = __ballot_sync(0xFFFFFFFFu, need != 0);
+    if (lanes) {  // (never without positional tables)
+      const int lead = __ffs(lanes) - 1, q0 = need ? __ffs(need) - 1 : 0;
+      u64 lh[4] = {h[0][0], h[0][1], h[0][2], h[0][3]};
+      bool lfit = hfit[0];
+#pragma unroll
+      for (int q = 1; q < SPT; q++)
+        if (q == q0) lh[0] = h[q][0], lh[1] = h[q][1], lh[2] = h[q][2], lh[3] = h[q][3], lfit = hfit[q];
+#pragma unroll
+      for (int j = 0; j < 4; j++) lh[j] = __shfl_sync(0xFFFFFFFFu, lh[j], lead);
+      lfit = __shfl_sync(0xFFFFFFFFu, (int)lfit, lead) != 0;
+      u32 lhead = 0, llen = 0;
+      int ln = heads_probe(t.bytecode, Fr{{lh[0], lh[1], lfit ? 0ull : 1ull, 0}}, Fr{{lh[2], lh[3], 0, 0}}, &lhead, &llen,
+                           1u << lane, (int)lane == lead);
+      ln = __shfl_sync(0xFFFFFFFFu, ln, lead);
+      lhead = __shfl_sync(0xFFFFFFFFu, lhead, lead);
+      llen = __shfl_sync(0xFFFFFFFFu, llen, lead);
+      bool peek[SPT];
+      u64 row[SPT];
+#pragma unroll
+      for (int q = 0; q < SPT; q++) {
+        int nh = ln;
+        u32 head = lhead, len = llen;
+        if ((need >> q & 1) && !(hfit[q] == lfit && h[q][0] == lh[0] && h[q][1] == lh[1] && h[q][2] == lh[2] && h[q][3] == lh[3]))
+          nh = heads_probe(t.bytecode, Fr{{h[q][0], h[q][1], hfit[q] ? 0ull : 1ull, 0}}, Fr{{h[q][2], h[q][3], 0, 0}}, &head, &len,
+                           1u << lane, true);
+        peek[q] = (need >> q & 1) && mul_peek_row(nh, head, len, pc[q], &row[q]);
+      }
+      Fr v[SPT];
+#pragma unroll
+      for (int q = 0; q < SPT; q++) v[q] = table_cell(t.bytecode.tab, B_VALUE, peek[q] ? row[q] : 0);  // loads first
+#pragma unroll
+      for (int q = 0; q < SPT; q++)
+        if (peek[q]) b[q] = mul_peek_bucket(v[q]);
+    }
+#pragma unroll
+    for (int q = 0; q < SPT; q++) {
+      const u64 k = base + (u64)q * ZK_SORT_THREADS + threadIdx.x;
+      if (k < n) so.bucket[k] = (unsigned char)b[q];
+      // lanes of a warp that share a bucket elect a leader, leaders add to the block's histogram
+      const unsigned m = __match_any_sync(0xFFFFFFFFu, b[q]);
+      if (b[q] != ZK_BK_NONE && lane == (unsigned)(__ffs(m) - 1)) atomicAdd(&s_hist[b[q]], (u32)__popc(m));
+    }
   }
-  const unsigned m = __match_any_sync(0xFFFFFFFFu, b);
-  if (b != ZK_BK_NONE && lane == (unsigned)(__ffs(m) - 1)) atomicAdd(&s_hist[b], (u32)__popc(m));
   __syncthreads();
   if (threadIdx.x < ZK_EVM_NB && s_hist[threadIdx.x]) atomicAdd(&so.hist[threadIdx.x], s_hist[threadIdx.x]);
   if (blockIdx.x == 0 && threadIdx.x == 0) so.hist[ZK_EVM_NB] = pos ? 1u : 0u;
-  // the last block to finish writes the whole histogram straight into the host's pinned buffer: the host reads it once
-  // this kernel is complete, and k_evm_scatter starts without waiting for a device-to-host copy
-  // (one fence per block, by the thread that counts the block: the barrier orders the block's histogram atomics before it)
-  __shared__ bool s_last;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    s_last = atomicAdd(so.done, 1u) == gridDim.x - 1;
-  }
-  __syncthreads();
-  if (s_last) {
-    __threadfence();
-    if (threadIdx.x <= ZK_EVM_NB) so.host_hist[threadIdx.x] = __ldcg(&so.hist[threadIdx.x]);
-  }
-}
+  grid.sync();
 
-__global__ void __launch_bounds__(1024) k_evm_scatter(EvmSort so, u32 n) {
-  __shared__ u32 s_off[ZK_EVM_NB + 1], s_cnt[ZK_EVM_NB], s_base[ZK_EVM_NB], s_wsum[ZK_EVM_NB / 32];
-  const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (blockIdx.x == 0) {  // publish: histogram + flag, a system-scope fence by every writer, then the sequence number
+    if (threadIdx.x <= ZK_EVM_NB) {
+      so.host_hist[threadIdx.x] = __ldcg(&so.hist[threadIdx.x]);
+      __threadfence_system();
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) *(volatile u32*)&so.host_hist[ZK_EVM_NB + 1] = seq;
+  }
   if (threadIdx.x < ZK_EVM_NB) {  // exclusive scan of the histogram (4 warps)
-    const u32 c = so.hist[threadIdx.x];
+    const u32 c = __ldcg(&so.hist[threadIdx.x]);
     u32 v = c;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
@@ -2025,29 +2100,34 @@ __global__ void __launch_bounds__(1024) k_evm_scatter(EvmSort so, u32 n) {
     }
     if (lane == 31) s_wsum[warp] = v;
     s_off[threadIdx.x] = v - c;
-    s_cnt[threadIdx.x] = 0;
   }
   __syncthreads();
   if (threadIdx.x < ZK_EVM_NB) {
     u32 add = 0;
     for (unsigned q = 0; q < warp; q++) add += s_wsum[q];
     s_off[threadIdx.x] += add;
-    if (threadIdx.x == ZK_EVM_NB - 1) s_off[ZK_EVM_NB] = s_off[threadIdx.x] + so.hist[threadIdx.x];
+    if (threadIdx.x == ZK_EVM_NB - 1) s_off[ZK_EVM_NB] = s_off[threadIdx.x] + __ldcg(&so.hist[threadIdx.x]);
+    if (s_hist[threadIdx.x]) s_hist[threadIdx.x] = s_off[threadIdx.x] + atomicAdd(&so.cursor[threadIdx.x], s_hist[threadIdx.x]);
   }
-  const u32 k = blockIdx.x * blockDim.x + threadIdx.x;
-  const int b = k < n ? (int)so.bucket[k] : ZK_BK_NONE;
-  const unsigned m = __match_any_sync(0xFFFFFFFFu, b);
-  const int leader = __ffs(m) - 1;
-  const u32 rank = __popc(m & ((1u << lane) - 1));
   __syncthreads();
-  u32 wbase = 0;
-  if (b != ZK_BK_NONE && (int)lane == leader) wbase = atomicAdd(&s_cnt[b], (u32)__popc(m));
-  wbase = __shfl_sync(0xFFFFFFFFu, wbase, leader);
-  __syncthreads();
-  if (threadIdx.x < ZK_EVM_NB && s_cnt[threadIdx.x]) s_base[threadIdx.x] = atomicAdd(&so.cursor[threadIdx.x], s_cnt[threadIdx.x]);
-  __syncthreads();
-  if (b != ZK_BK_NONE) so.sorted[s_off[b] + s_base[b] + wbase + rank] = k;
   if (blockIdx.x == 0 && threadIdx.x <= ZK_EVM_NB) so.offs[threadIdx.x] = s_off[threadIdx.x];
+  for (u64 base = (u64)blockIdx.x * TILE; base < n; base += (u64)gridDim.x * TILE) {
+    int b[SPT];
+#pragma unroll
+    for (int q = 0; q < SPT; q++) {
+      const u64 k = base + (u64)q * ZK_SORT_THREADS + threadIdx.x;
+      b[q] = k < n ? (int)__ldcg(&so.bucket[k]) : ZK_BK_NONE;
+    }
+#pragma unroll
+    for (int q = 0; q < SPT; q++) {
+      const unsigned m = __match_any_sync(0xFFFFFFFFu, b[q]);
+      const int leader = __ffs(m) - 1;
+      u32 wbase = 0;
+      if (b[q] != ZK_BK_NONE && (int)lane == leader) wbase = atomicAdd(&s_hist[b[q]], (u32)__popc(m));
+      wbase = __shfl_sync(0xFFFFFFFFu, wbase, leader);
+      if (b[q] != ZK_BK_NONE) so.sorted[wbase + __popc(m & ((1u << lane) - 1))] = (u32)(base + (u64)q * ZK_SORT_THREADS + threadIdx.x);
+    }
+  }
 }
 
 // Work queue of the hot kernels (k_evm_gadget, k_evm_push_*): a group's buckets are cut into chunks of 32
