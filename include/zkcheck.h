@@ -234,16 +234,30 @@ int zk_assign_keccak_table(zk_ctx* ctx, uint64_t n, const uint8_t* data, const u
  *   at or beyond src_addr_end), is_code_bits = one bit per data byte (events that touch bytecode; may be NULL).
  *   Two rows per byte (read row, write row) incl. rlc_acc under ZK_CHALLENGE_KECCAK, rw_counter / rwc_inc_left and
  *   the id type flags.
+ * zk_assign_exp_circuit = ExpCircuit.add_event per event, then fill_dummy_events (evm_circuit/typing.py:880-994), and
+ *   the exp table the EVM circuit's EXP lookups read (Tables._convert_exp_circuit_to_table, table.py:654-671):
+ *   events[n][12] = { base (4 little-endian limbs), exponent (4 limbs), identifier (4 limbs, canonical Fr) }.
+ *   ZK_CIRCUIT_EXP becomes the rows of every event in order ((bitlen(x) - 1) + (popcount(x) - 1) rows for an exponent
+ *   x >= 2, none for 0 and 1), padded with the constant dummy row up to n_rows_min rows when that is larger.
+ *   ZK_TABLE_EXP becomes one row per event row, plus the padding row (is_step 1, identifier 0, is_last 0, base 1,
+ *   exponent 1, exponentiation 1) once if any padding was written; indexes cached on the old table are dropped.
+ *   n_events = 0 is valid.  An identifier >= p, or n_rows_min or the event rows reaching 2^31 - 1, returns -1 before
+ *   anything is stored: the previous matrix and table stay in place.
  * zk_download_columns widens the resident matrix of a circuit back to canonical cells
- *   (colmajor_out: uint64[n_cols][zk_resident_rows][4]; flags_out: uint8[rows] or NULL) — inspection and tests. */
+ *   (colmajor_out: uint64[n_cols][zk_resident_rows][4]; flags_out: uint8[rows] or NULL) — inspection and tests.
+ *   zk_table_rows / zk_download_table do the same for a resident lookup table
+ *   (colmajor_out: uint64[zk_table_cols][zk_table_rows][4]). */
 int zk_assign_bytecode_circuit(zk_ctx* ctx, uint32_t k, uint64_t n_contracts, const uint8_t* code, const uint8_t* is_code_bits,
                                const uint64_t* code_offsets, const uint64_t* hashes, void* stream);
 int zk_assign_state_circuit(zk_ctx* ctx, uint64_t n_rows, const void* packed_ops, uint64_t total_bytes,
                             const uint64_t* col_offsets, const uint8_t* col_widths, const uint8_t* row_flags, void* stream);
 int zk_assign_copy_circuit(zk_ctx* ctx, uint64_t n_events, const uint64_t* events, const uint8_t* data,
                            const uint8_t* is_code_bits, void* stream);
+int zk_assign_exp_circuit(zk_ctx* ctx, uint64_t n_events, const uint64_t* events, uint64_t n_rows_min, void* stream);
 int64_t zk_resident_rows(zk_ctx* ctx, int circuit_id);
 int zk_download_columns(zk_ctx* ctx, int circuit_id, uint64_t* colmajor_out, uint8_t* flags_out, void* stream);
+int64_t zk_table_rows(zk_ctx* ctx, int table_id);
+int zk_download_table(zk_ctx* ctx, int table_id, uint64_t* colmajor_out, void* stream);
 
 /* Check rows [row_begin, row_end) of the resident matrix (local indices).  Without
  * ZK_FLAG_WRAP the caller guarantees halo rows exist for the circuit's rotations.

@@ -1,9 +1,10 @@
 """Witness assignment on the device — host side of include/zkcheck.h "witness assignment" (csrc/assign.cu).
 
 The reference builds circuit rows with Python object loops (assign_bytecode_circuit, bytecode_circuit.py:104-167;
-op2row / assign_state_circuit, state_circuit.py:827-889; CopyCircuit.copy, evm_circuit/typing.py:1010-1147).  The
-functions here hand the device the compact data those loops start from — raw code bytes, 15 operation cells, copy
-events + the copied bytes — and leave the expanded witness resident for zk_check."""
+op2row / assign_state_circuit, state_circuit.py:827-889; CopyCircuit.copy, evm_circuit/typing.py:1010-1147;
+ExpCircuit.add_event, evm_circuit/typing.py:880-994).  The functions here hand the device the compact data those loops
+start from — raw code bytes, 15 operation cells, copy events + the copied bytes, (base, exponent, identifier) per
+exponentiation — and leave the expanded witness resident for zk_check."""
 from __future__ import annotations
 
 from typing import Dict, List, Optional, Sequence
@@ -99,3 +100,26 @@ def assign_copy_circuit(ctx: native.Context, r, events: Sequence[Sequence[int]],
     if is_code is not None:
         bits = np.packbits(np.asarray(is_code, dtype=np.uint8), bitorder="little") if len(data) else np.zeros(1, dtype=np.uint8)
     ctx.assign_copy_circuit(ev, np.frombuffer(bytes(data), dtype=np.uint8), bits, stream=stream)
+
+
+def exp_events(triples) -> np.ndarray:
+    """(base, exponent, identifier) per ExpCircuit.add_event -> the uint64[n][12] events of zk_assign_exp_circuit.  Base
+    and exponent become Words as in the reference (an int outside [0, 2^256) raises there, and here); the identifier is
+    reduced mod p like FQ()"""
+    M = (1 << 64) - 1
+    out = np.zeros((len(triples), 12), dtype=np.uint64)
+    for k, (base, exponent, identifier) in enumerate(triples):
+        ident = FQ(packing.cell_int(identifier)).n
+        for j, v in enumerate((Word(int(base)).int_value(), Word(int(exponent)).int_value(), ident)):
+            out[k, 4 * j:4 * j + 4] = [(v >> (64 * i)) & M for i in range(4)]
+    return out
+
+
+def assign_exp_circuit(ctx: native.Context, triples, max_exp_steps: Optional[int] = None, stream: int = 0) -> None:
+    """ExpCircuit(max_exp_steps).add_event(...) for every (base, exponent, identifier), then fill_dummy_events() when
+    max_exp_steps is given, as one device call: the rows stay resident as ZK_CIRCUIT_EXP, the exp table the EVM circuit's
+    EXP lookups read (Tables(exp_circuit=...)) as ZK_TABLE_EXP"""
+    from .exp_circuit import ExpCircuit
+
+    n_min = 0 if max_exp_steps is None else int(max_exp_steps) * ExpCircuit.OFFSET_INCREMENT
+    ctx.assign_exp_circuit(exp_events(list(triples)), n_rows_min=n_min, stream=stream)

@@ -866,17 +866,60 @@ extern "C" int zk_assign_copy_circuit(zk_ctx* ctx, uint64_t n_events, const uint
   return launched(ctx, "k_assign_copy_rows");
 }
 
+template <class K>
+static unsigned grid_persistent(zk_ctx* ctx, K kernel, int threads, u64 n_items);
+extern "C" int zk_assign_exp_circuit(zk_ctx* ctx, uint64_t n_events, const uint64_t* events, uint64_t n_rows_min, void* stream) {
+  CK(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  // everything is validated before the resident matrix or table is touched: a rejected call leaves both in place
+  std::vector<u64> row_off(n_events + 1, 0);
+  for (u64 e = 0; e < n_events; e++) {
+    if (!fr_is_canonical((const u64*)events + 12 * e + 8)) return fail_msg(ctx, "exp event identifier is not canonical (>= p)");
+    row_off[e + 1] = row_off[e] + exp_event_rows((const u64*)events + 12 * e + 4);
+  }
+  const u64 n_used = row_off[n_events], n_rows = std::max<u64>(n_used, n_rows_min);
+  if (n_rows >= 0x7FFFFFFFull) return fail_msg(ctx, "too many exp rows (the exp table holds one row per circuit row)");
+  const u64 n_table = n_used + (n_rows > n_used ? 1 : 0);
+  const size_t s_ev = 0, s_off = up32(n_events * 96), s_total = s_off + (n_events + 1) * 8;
+  int rc;
+  if ((rc = ensure_astage(ctx, s_total))) return rc;
+  unsigned char* sg = ctx->astage;
+  if (n_events) CK(ctx, cudaMemcpyAsync(sg + s_ev, events, n_events * 96, cudaMemcpyHostToDevice, st));
+  CK(ctx, cudaMemcpyAsync(sg + s_off, row_off.data(), (n_events + 1) * 8, cudaMemcpyHostToDevice, st));
+  Matrix& m = ctx->circ[ZK_CIRCUIT_EXP];
+  Matrix& t = ctx->tab[ZK_TABLE_EXP];
+  if ((rc = alloc_narrow(ctx, m, n_rows, 21, kExpAssignWidths))) return rc;
+  if ((rc = alloc_narrow(ctx, t, n_table, 11, kExpTableWidths))) return rc;  // a new version: cached indexes are rebuilt
+  if (n_rows == 0) return 0;
+  ExpAssign a;
+  a.ev = (const u64*)(sg + s_ev);
+  a.row_off = (const u64*)(sg + s_off);
+  a.n_events = n_events, a.n_used = n_used, a.n_rows = n_rows;
+  a.base = (unsigned char*)m.dev;
+  a.tbase = (unsigned char*)t.dev;
+  for (int c = 0; c < 21; c++) a.off[c] = m.off[c];
+  for (int c = 0; c < 11; c++) a.toff[c] = t.off[c];
+  int n_launch = 1;
+  if (n_used) {
+    k_assign_exp_chain<<<(unsigned)((n_events + 127) / 128), 128, 0, st>>>(a);
+    n_launch = 2;
+  }
+  k_assign_exp_rows<<<grid_persistent(ctx, k_assign_exp_rows, 256, n_rows), 256, 0, st>>>(a);
+  return launched(ctx, "k_assign_exp_chain / k_assign_exp_rows", n_launch);
+}
+
 extern "C" int64_t zk_resident_rows(zk_ctx* ctx, int circuit_id) {
   if (circuit_id < 0 || circuit_id >= ZK_N_CIRCUITS) return -1;
   return (int64_t)ctx->circ[circuit_id].n_rows;
 }
+extern "C" int64_t zk_table_rows(zk_ctx* ctx, int table_id) {
+  if (table_id < 0 || table_id >= ZK_N_TABLES) return -1;
+  return (int64_t)ctx->tab[table_id].n_rows;
+}
 
-// the resident matrix of a circuit widened back to canonical cells on the host (inspection / tests)
-extern "C" int zk_download_columns(zk_ctx* ctx, int circuit_id, uint64_t* colmajor_out, uint8_t* flags_out, void* stream) {
-  if (circuit_id < 0 || circuit_id >= ZK_N_CIRCUITS) return fail_msg(ctx, "bad circuit id");
+// a resident matrix widened back to canonical cells on the host (inspection / tests)
+static int download_matrix(zk_ctx* ctx, const Matrix& m, uint64_t* colmajor_out, uint8_t* flags_out, cudaStream_t st) {
   CK(ctx, cudaSetDevice(ctx->device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const Matrix& m = ctx->circ[circuit_id];
   CK(ctx, cudaStreamSynchronize(st));
   std::vector<unsigned char> tmp;
   for (u32 c = 0; c < m.n_cols; c++) {
@@ -896,6 +939,14 @@ extern "C" int zk_download_columns(zk_ctx* ctx, int circuit_id, uint64_t* colmaj
     else memset(flags_out, 0, m.n_rows);
   }
   return 0;
+}
+extern "C" int zk_download_columns(zk_ctx* ctx, int circuit_id, uint64_t* colmajor_out, uint8_t* flags_out, void* stream) {
+  if (circuit_id < 0 || circuit_id >= ZK_N_CIRCUITS) return fail_msg(ctx, "bad circuit id");
+  return download_matrix(ctx, ctx->circ[circuit_id], colmajor_out, flags_out, (cudaStream_t)stream);
+}
+extern "C" int zk_download_table(zk_ctx* ctx, int table_id, uint64_t* colmajor_out, void* stream) {
+  if (table_id < 0 || table_id >= ZK_N_TABLES) return fail_msg(ctx, "bad table id");
+  return download_matrix(ctx, ctx->tab[table_id], colmajor_out, nullptr, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------ lookup index cache

@@ -4,6 +4,8 @@
 //   assign_bytecode_circuit  src/zkevm_specs/bytecode_circuit.py:104-167   raw code bytes -> 12-cell rows
 //   op2row / assign_state_circuit  src/zkevm_specs/state_circuit.py:827-889  15 operation cells -> 57-cell rows
 //   CopyCircuit.copy         src/zkevm_specs/evm_circuit/typing.py:1010-1147 copy events + bytes -> 20-cell rows
+//   ExpCircuit.add_event     src/zkevm_specs/evm_circuit/typing.py:880-994  (base, exponent, id) -> 21-cell rows
+//                            + the exp table (Tables._convert_exp_circuit_to_table, table.py:654-671)
 //
 // The two sequential pieces — value_rlc of a contract and rlc_acc of a copy event, both Horner chains
 // acc = acc * r + byte — run as a chunked segmented scan: one thread folds a 32-byte chunk
@@ -13,6 +15,7 @@
 // (fr.cuh:ld_col widths), so a check after an assignment reads 80-150 B per row instead of 384-1,824.
 // Included by api.cu (it uses the context).
 #include "circuit.cuh"
+#include "words.cuh"
 
 namespace zk {
 
@@ -289,6 +292,176 @@ ZK_HD void assign_copy_chunk(const CopyAssign& a, const Fr* chunk_val, const Fr*
   }
 }
 
+// ---------------------------------------------------------------- exponentiation circuit
+// one event = ExpCircuit.add_event(base, exponent, identifier): n = (bitlen(x) - 1) + (popcount(x) - 1) rows for an
+// exponent x >= 2 (none for 0 and 1), row 0 the final product.  Counted from the top, e_0 = x and e_{k+1} = e_k - 1
+// (e_k odd) or e_k / 2; d_k = base^e_k mod 2^256, a_k = d_{k+1} (a_{n-1} = base), b_k = base (e_k odd) or a_k.
+// Only d is a chain: k_assign_exp_chain runs square-and-multiply per event and writes d of each row it produces;
+// every other cell is a closed form of (x, k, base, identifier, d_k, d_{k+1}).  Walking x from its least significant
+// bit, bit j < bitlen(x) - 1 contributes an odd row e = x >> j when it is set, then an even row e = (x >> j) & ~1, so
+// j + popcount(x mod 2^j) rows precede bit j's rows.
+struct ExpAssign {
+  const u64* ev;       // [n_events][12]: base, exponent, identifier (4 little-endian limbs each)
+  const u64* row_off;  // [n_events + 1] first row of each event
+  u64 n_events, n_used, n_rows;  // event rows, circuit rows (n_used + fill_dummy_events padding)
+  unsigned char* base;  // the circuit's narrow columns
+  u64 off[21];
+  unsigned char* tbase;  // the exp table's narrow columns: n_used rows, + the padding row once if n_rows > n_used
+  u64 toff[11];
+};
+static const unsigned char kExpAssignWidths[21] = {1, 1, 32, 1, 16, 16, 16, 16, 16, 16, 16, 16, 16, 16, 1, 1, 16, 16, 16, 16, 1};
+static const unsigned char kExpTableWidths[11] = {1, 32, 1, 8, 8, 8, 8, 16, 16, 16, 16};
+enum { E_USABLE, E_STEP, E_ID, E_LAST, E_BASE, E_EXPO = 6, E_EXPN = 8, E_A = 10, E_B = 12, E_C = 14, E_D = 16, E_Q = 18, E_R = 20 };
+
+ZK_HD int zk_popc64(u64 x) {
+#ifdef __CUDA_ARCH__
+  return __popcll(x);
+#else
+  return __builtin_popcountll(x);
+#endif
+}
+ZK_HD int zk_bitlen64(u64 x) {
+#ifdef __CUDA_ARCH__
+  return 64 - __clzll((long long)x);
+#else
+  return x ? 64 - __builtin_clzll(x) : 0;
+#endif
+}
+ZK_HD int exp_bitlen(const u64 x[4]) {
+  return x[3] ? 192 + zk_bitlen64(x[3]) : x[2] ? 128 + zk_bitlen64(x[2]) : x[1] ? 64 + zk_bitlen64(x[1]) : zk_bitlen64(x[0]);
+}
+// rows of one event (the host sizes the circuit with it)
+ZK_HD u64 exp_event_rows(const u64 x[4]) {
+  const int len = exp_bitlen(x);
+  if (len < 2) return 0;
+  return (u64)(len - 1) + (u64)(zk_popc64(x[0]) + zk_popc64(x[1]) + zk_popc64(x[2]) + zk_popc64(x[3]) - 1);
+}
+// limb i of x (0 beyond the top), without indexing x by a run-time value (which would put it in local memory)
+ZK_HD u64 limb_at(const u64 x[4], int i) { return i == 0 ? x[0] : i == 1 ? x[1] : i == 2 ? x[2] : i == 3 ? x[3] : 0; }
+// popcount(x mod 2^j), 0 <= j <= 256
+ZK_HD int popc_below(const u64 x[4], int j) {
+  int n = 0;
+#pragma unroll
+  for (int i = 0; i < 4; i++) {
+    const int b = j - 64 * i;
+    const u64 m = b >= 64 ? ~0ull : (b <= 0 ? 0ull : (1ull << b) - 1);
+    n += zk_popc64(x[i] & m);
+  }
+  return n;
+}
+
+// d of every row of event k: forward step f (from the top bit down) produces row n - 1 - f
+ZK_HD void assign_exp_chain(const ExpAssign& a, u64 k) {
+  const u64* e = a.ev + 12 * k;
+  const u64 b[4] = {e[0], e[1], e[2], e[3]}, x[4] = {e[4], e[5], e[6], e[7]};
+  const u64 r0 = a.row_off[k], n = a.row_off[k + 1] - r0;
+  if (n == 0) return;
+  unsigned char* dlo = a.base + a.off[E_D];
+  unsigned char* dhi = a.base + a.off[E_D + 1];
+  u64 acc[4] = {b[0], b[1], b[2], b[3]};
+  u64 row = r0 + n;
+  for (int j = exp_bitlen(x) - 2; j >= 0; j--) {
+    mul256_lo(acc, acc, acc);  // square: e = 2 e
+    row--;
+    st_u128(dlo, row, acc[0], acc[1]);
+    st_u128(dhi, row, acc[2], acc[3]);
+    if ((limb_at(x, j >> 6) >> (j & 63)) & 1) {  // multiply: e = e + 1
+      mul256_lo(acc, b, acc);
+      row--;
+      st_u128(dlo, row, acc[0], acc[1]);
+      st_u128(dhi, row, acc[2], acc[3]);
+    }
+  }
+}
+
+// every other cell of circuit row r, and table row r (+ the padding row at n_used)
+ZK_HD void assign_exp_row(const ExpAssign& a, u64 r) {
+  unsigned char* B = a.base;
+  u64 b[4] = {1, 0, 0, 0}, ex[4] = {1, 0, 0, 0}, id[4] = {0, 0, 0, 0}, q[4] = {0, 0, 0, 0}, d[4] = {1, 0, 0, 0}, m[4];
+  u64 odd = 1;
+  bool step = false, last = false;
+  if (r < a.n_used) {
+    u64 lo = 0, hi = a.n_events;  // the largest k with row_off[k] <= r: the event (with rows) that holds row r
+    while (hi - lo > 1) {
+      const u64 mid = (lo + hi) >> 1;
+      if (a.row_off[mid] <= r) lo = mid;
+      else hi = mid;
+    }
+    const u64* e = a.ev + 12 * lo;
+    const u64 x[4] = {e[4], e[5], e[6], e[7]};
+    b[0] = e[0], b[1] = e[1], b[2] = e[2], b[3] = e[3];
+    id[0] = e[8], id[1] = e[9], id[2] = e[10], id[3] = e[11];
+    const u64 k = r - a.row_off[lo];
+    last = r + 1 == a.row_off[lo + 1];
+    step = true;
+    // the bit j whose rows hold row k: the largest j < bitlen(x) - 1 with j + popcount(x mod 2^j) <= k
+    int jl = 0, jh = exp_bitlen(x) - 1;
+    while (jh - jl > 1) {
+      const int mid = (jl + jh) >> 1;
+      if ((u64)(mid + popc_below(x, mid)) <= k) jl = mid;
+      else jh = mid;
+    }
+    const int sh = jl >> 6, bt = jl & 63;
+#pragma unroll
+    for (int i = 0; i < 4; i++) {  // e = x >> j
+      const u64 l0 = limb_at(x, i + sh), l1 = limb_at(x, i + sh + 1);
+      ex[i] = bt ? (l0 >> bt) | (l1 << (64 - bt)) : l0;
+    }
+    odd = (ex[0] & 1) && k == (u64)(jl + popc_below(x, jl));
+    ex[0] &= odd ? ~0ull : ~1ull;
+#pragma unroll
+    for (int i = 0; i < 4; i++) q[i] = (ex[i] >> 1) | (i < 3 ? ex[i + 1] << 63 : 0);
+    const u64* dl = (const u64*)(B + a.off[E_D]);
+    const u64* dh = (const u64*)(B + a.off[E_D + 1]);
+    d[0] = dl[2 * r], d[1] = dl[2 * r + 1], d[2] = dh[2 * r], d[3] = dh[2 * r + 1];
+    if (last) {
+      m[0] = b[0], m[1] = b[1], m[2] = b[2], m[3] = b[3];
+    } else {
+      m[0] = dl[2 * r + 2], m[1] = dl[2 * r + 3], m[2] = dh[2 * r + 2], m[3] = dh[2 * r + 3];
+    }
+  } else {  // fill_dummy_events: (1, 0, 0, 0, base 1, exponent 1, exponentiation 1, a 1, b 1, c 0, d 1, q 0, r 1)
+    m[0] = 1, m[1] = m[2] = m[3] = 0;
+    st_u128(B + a.off[E_D], r, 1, 0);
+    st_u128(B + a.off[E_D + 1], r, 0, 0);
+  }
+  u64 bb[4];  // b = base (odd) or a, chosen cell by cell: a pointer to either array would put both in local memory
+#pragma unroll
+  for (int i = 0; i < 4; i++) bb[i] = odd ? b[i] : m[i];
+  B[a.off[E_USABLE] + r] = 1;
+  B[a.off[E_STEP] + r] = step;
+  st_fr(B + a.off[E_ID], r, Fr{{id[0], id[1], id[2], id[3]}});
+  B[a.off[E_LAST] + r] = last;
+  st_u128(B + a.off[E_BASE], r, b[0], b[1]);
+  st_u128(B + a.off[E_BASE + 1], r, b[2], b[3]);
+  st_u128(B + a.off[E_EXPO], r, ex[0], ex[1]);
+  st_u128(B + a.off[E_EXPO + 1], r, ex[2], ex[3]);
+  st_u128(B + a.off[E_EXPN], r, d[0], d[1]);
+  st_u128(B + a.off[E_EXPN + 1], r, d[2], d[3]);
+  st_u128(B + a.off[E_A], r, m[0], m[1]);
+  st_u128(B + a.off[E_A + 1], r, m[2], m[3]);
+  st_u128(B + a.off[E_B], r, bb[0], bb[1]);
+  st_u128(B + a.off[E_B + 1], r, bb[2], bb[3]);
+  B[a.off[E_C] + r] = 0;
+  B[a.off[E_C + 1] + r] = 0;
+  st_u128(B + a.off[E_Q], r, q[0], q[1]);
+  st_u128(B + a.off[E_Q + 1], r, q[2], q[3]);
+  B[a.off[E_R] + r] = (unsigned char)odd;
+  // the table row (Tables._convert_exp_circuit_to_table: is_step = 1 on every row, padding included): one per event
+  // row, and the padding row once, at n_used
+  if (r <= a.n_used) {
+    unsigned char* T = a.tbase;
+    T[a.toff[0] + r] = 1;
+    st_fr(T + a.toff[1], r, Fr{{id[0], id[1], id[2], id[3]}});
+    T[a.toff[2] + r] = last;
+#pragma unroll
+    for (int i = 0; i < 4; i++) ((u64*)(T + a.toff[3 + i]))[r] = b[i];
+    st_u128(T + a.toff[7], r, ex[0], ex[1]);
+    st_u128(T + a.toff[8], r, ex[2], ex[3]);
+    st_u128(T + a.toff[9], r, d[0], d[1]);
+    st_u128(T + a.toff[10], r, d[2], d[3]);
+  }
+}
+
 #ifdef __CUDACC__
 __global__ void __launch_bounds__(256) k_seg_local(SegHorner s, Fr* chunk_val) {
   const u64 c = (u64)blockIdx.x * blockDim.x + threadIdx.x;
@@ -313,6 +486,15 @@ __global__ void __launch_bounds__(256) k_assign_state_derive(const __grid_consta
 __global__ void __launch_bounds__(256) k_assign_copy_rows(const __grid_constant__ CopyAssign a, const Fr* chunk_val, const Fr* seg_total) {
   const u64 c = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (c < a.s.n_chunks) assign_copy_chunk(a, chunk_val, seg_total, c);
+}
+__global__ void __launch_bounds__(128) k_assign_exp_chain(const __grid_constant__ ExpAssign a) {
+  const u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < a.n_events) assign_exp_chain(a, k);
+}
+// persistent grid (api.cu grid_persistent): threads walk the rows with a grid stride
+__global__ void __launch_bounds__(256) k_assign_exp_rows(const __grid_constant__ ExpAssign a) {
+  const u64 stride = (u64)gridDim.x * blockDim.x;
+  for (u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x; r < a.n_rows; r += stride) assign_exp_row(a, r);
 }
 #endif
 

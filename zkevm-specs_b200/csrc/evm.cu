@@ -647,22 +647,6 @@ ZK_HD bool word_select(const Word2& w, const Fr& sel, Word2* out) {
   return word_in_domain(*out);
 }
 
-// low 256 bits of a * b
-ZK_HD void mul256_lo(const u64 a[4], const u64 b[4], u64 o[4]) {
-  u64 t[4] = {0, 0, 0, 0};
-#pragma unroll
-  for (int x = 0; x < 4; x++) {
-    u64 c = 0;
-#pragma unroll
-    for (int y = 0; y + x < 4; y++) {
-      unsigned __int128 v = (unsigned __int128)a[x] * b[y] + t[x + y] + c;
-      t[x + y] = (u64)v;
-      c = (u64)(v >> 64);
-    }
-  }
-#pragma unroll
-  for (int k = 0; k < 4; k++) o[k] = t[k];
-}
 // MUL / DIV / MOD decided as a whole for stack words in the halves domain: true iff every constraint of
 // mul_div_mod.py:23-64 holds.  In that domain the gate a * b + c == d (+ the 9-byte carries, overflow == 0 for
 // DIV / MOD), the select equation and remainder < divisor are statements about 256-bit integers:

@@ -2,7 +2,7 @@
 //
 // Device-side counterpart of Word (src/zkevm_specs/util/arithmetic.py:99-168) and of
 // mul_add_words (util/arithmetic.py:245-276, evm_circuit/instruction.py:599-632), shared by the
-// MUL/DIV/MOD gate program (evm.cu) and the exp circuit (exp.cu).
+// MUL/DIV/MOD gate program (evm.cu), the exp circuit (exp.cu) and its row builder (assign.cu).
 #pragma once
 #include "fr.cuh"
 
@@ -68,5 +68,23 @@ ZK_HD void mul_add_carries(const Word2& a, const Word2& b, const Word2& c, const
 }
 // range_check(x, 9): x.n fits 9 bytes
 ZK_HD bool fits_9_bytes(const Fr& x) { return fr_fits128(x) && (x.l[1] >> 8) == 0; }
+
+// low 256 bits of a * b (4 little-endian limbs): the MUL gate's fast form (evm.cu) and the exp circuit's
+// square-and-multiply chain (assign.cu)
+ZK_HD void mul256_lo(const u64 a[4], const u64 b[4], u64 o[4]) {
+  u64 t[4] = {0, 0, 0, 0};
+#pragma unroll
+  for (int x = 0; x < 4; x++) {
+    u64 c = 0;
+#pragma unroll
+    for (int y = 0; y + x < 4; y++) {
+      unsigned __int128 v = (unsigned __int128)a[x] * b[y] + t[x + y] + c;
+      t[x + y] = (u64)v;
+      c = (u64)(v >> 64);
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 4; k++) o[k] = t[k];
+}
 
 }  // namespace zk

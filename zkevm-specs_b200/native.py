@@ -75,7 +75,8 @@ EXPORTS = [
     "zk_last_timing", "zk_upload_columns_packed", "zk_upload_table_packed",
     "zk_upload_bytecode_table_from_code", "zk_nccl_unique_id", "zk_nccl_comm_init", "zk_nccl_comm_destroy",
     "zk_keccak256_batch", "zk_assign_keccak_table", "zk_assign_bytecode_circuit", "zk_assign_state_circuit",
-    "zk_assign_copy_circuit", "zk_download_columns", "zk_resident_rows",
+    "zk_assign_copy_circuit", "zk_download_columns", "zk_resident_rows", "zk_assign_exp_circuit", "zk_table_rows",
+    "zk_download_table",
 ]
 
 
@@ -117,6 +118,10 @@ def lib() -> ctypes.CDLL:
         L.zk_download_columns.argtypes = [vp, i32, vp, vp, vp]
         L.zk_resident_rows.argtypes = [vp, i32]
         L.zk_resident_rows.restype = ctypes.c_int64
+        L.zk_assign_exp_circuit.argtypes = [vp, u64, vp, u64, vp]
+        L.zk_table_rows.argtypes = [vp, i32]
+        L.zk_table_rows.restype = ctypes.c_int64
+        L.zk_download_table.argtypes = [vp, i32, vp, vp]
         L.zk_circuit_cols.argtypes = [i32]
         L.zk_table_cols.argtypes = [i32]
         L.zk_n_constraints.argtypes = [i32]
@@ -288,6 +293,14 @@ class Context:
                                                 None if bits is None else _host_ptr(bits), ctypes.c_void_p(stream)),
                  "zk_assign_copy_circuit")
 
+    def assign_exp_circuit(self, events: np.ndarray, n_rows_min: int = 0, stream: int = 0) -> None:
+        """ExpCircuit.add_event per event + fill_dummy_events (evm_circuit/typing.py:880-994) on the device: `events`
+        uint64[n][12] = base, exponent, identifier (4 little-endian limbs each, the identifier canonical).  The rows stay
+        resident as ZK_CIRCUIT_EXP (padded to n_rows_min), their exp table as ZK_TABLE_EXP"""
+        ev = np.ascontiguousarray(events, dtype=np.uint64).reshape(-1, 12)
+        self._ck(self._L.zk_assign_exp_circuit(self._h, ev.shape[0], _host_ptr(ev), int(n_rows_min), ctypes.c_void_p(stream)),
+                 "zk_assign_exp_circuit")
+
     def download_columns(self, circuit_id: int, stream: int = 0):
         """the resident matrix of a circuit as canonical cells + its row flags: (uint64[n_cols][n_rows][4], uint8[n_rows])"""
         n_cols, n_rows = self._L.zk_circuit_cols(circuit_id), self.resident_rows(circuit_id)
@@ -299,6 +312,15 @@ class Context:
 
     def resident_rows(self, circuit_id: int) -> int:
         return int(self._L.zk_resident_rows(self._h, circuit_id))
+
+    def download_table(self, table_id: int, stream: int = 0) -> np.ndarray:
+        """a resident lookup table as canonical cells: uint64[n_cols][n_rows][4]"""
+        out = np.zeros((self._L.zk_table_cols(table_id), self.table_rows(table_id), 4), dtype=np.uint64)
+        self._ck(self._L.zk_download_table(self._h, table_id, _host_ptr(out), ctypes.c_void_p(stream)), "zk_download_table")
+        return out
+
+    def table_rows(self, table_id: int) -> int:
+        return int(self._L.zk_table_rows(self._h, table_id))
 
     def bind_columns_device(self, circuit_id: int, n_rows: int, n_cols: int, dev_ptr: int) -> None:
         self._ck(self._L.zk_bind_columns_device(self._h, circuit_id, n_rows, n_cols,
