@@ -243,6 +243,21 @@ int zk_assign_keccak_table(zk_ctx* ctx, uint64_t n, const uint8_t* data, const u
  *   exponent 1, exponentiation 1) once if any padding was written; indexes cached on the old table are dropped.
  *   n_events = 0 is valid.  An identifier >= p, or n_rows_min or the event rows reaching 2^31 - 1, returns -1 before
  *   anything is stored: the previous matrix and table stay in place.
+ * zk_assign_pi_circuit = public_data2witness (pi_circuit.py:839-1073) from the raw public-input stream
+ *   b"".join(rpi_byte_values) (n_bytes = circuit_len, one byte per row; the layout of pi_circuit.py:845-856 for the
+ *   three maxima).  ZK_CIRCUIT_PI becomes the n rows, as narrow columns; rpi_bytes_keccakrlc under
+ *   ZK_CHALLENGE_PI_KECCAK and rpi_value_lc under ZK_CHALLENGE_PI_BYTE_BASE, both read from the context;
+ *   ZK_PARAM_PI_CIRCUIT_LEN becomes n.  The call REPLACES the resident ZK_TABLE_KECCAK with the two rows the circuit
+ *   looks up, (0, 0, 0, 0, 0) and (1, rpi_bytes_keccakrlc of row 0, n, digest lo, hi), and ZK_TABLE_CALLDATA_GAS with
+ *   the zero row plus one (tx_id, is_final, gas_cost_acc) row per used calldata byte: the reference's set, whose padding
+ *   rows are copies of the zero row, without the copies; indexes cached on the old tables are dropped.  The digest is keccak256 of the bytes in the reference's
+ *   processing order (the values from last to first, each value's bytes first to last).  pi_keccak_out (or NULL):
+ *   the call synchronises `stream` and writes that digest as a Word (lo limb0, lo limb1, hi limb0, hi limb1).
+ *   Returns -1 before anything is stored (the previous rows, tables and circuit length stay in place) when
+ *   max_txs or max_withdrawals is 0, n_bytes is not the circuit_len of the three maxima, n_bytes >= 2^31 - 1, or the
+ *   max_txs CallDataLength fields (big-endian, at their fixed offsets) sum to more than max_calldata_bytes.  A stream
+ *   that is otherwise inconsistent (a CallDataGasCost that does not match the calldata, a zero withdrawal amount) is
+ *   assigned as it is, and zk_check decides whether it holds.
  * zk_download_columns widens the resident matrix of a circuit back to canonical cells
  *   (colmajor_out: uint64[n_cols][zk_resident_rows][4]; flags_out: uint8[rows] or NULL) — inspection and tests.
  *   zk_table_rows / zk_download_table do the same for a resident lookup table
@@ -254,6 +269,9 @@ int zk_assign_state_circuit(zk_ctx* ctx, uint64_t n_rows, const void* packed_ops
 int zk_assign_copy_circuit(zk_ctx* ctx, uint64_t n_events, const uint64_t* events, const uint8_t* data,
                            const uint8_t* is_code_bits, void* stream);
 int zk_assign_exp_circuit(zk_ctx* ctx, uint64_t n_events, const uint64_t* events, uint64_t n_rows_min, void* stream);
+int zk_assign_pi_circuit(zk_ctx* ctx, uint64_t max_txs, uint64_t max_calldata_bytes, uint64_t max_withdrawals,
+                         const uint8_t* raw_public_inputs, uint64_t n_bytes,
+                         uint64_t* pi_keccak_out /* [4]: lo limb0, lo limb1, hi limb0, hi limb1, or NULL */, void* stream);
 int64_t zk_resident_rows(zk_ctx* ctx, int circuit_id);
 int zk_download_columns(zk_ctx* ctx, int circuit_id, uint64_t* colmajor_out, uint8_t* flags_out, void* stream);
 int64_t zk_table_rows(zk_ctx* ctx, int table_id);

@@ -2,9 +2,10 @@
 
 The reference builds circuit rows with Python object loops (assign_bytecode_circuit, bytecode_circuit.py:104-167;
 op2row / assign_state_circuit, state_circuit.py:827-889; CopyCircuit.copy, evm_circuit/typing.py:1010-1147;
-ExpCircuit.add_event, evm_circuit/typing.py:880-994).  The functions here hand the device the compact data those loops
-start from — raw code bytes, 15 operation cells, copy events + the copied bytes, (base, exponent, identifier) per
-exponentiation — and leave the expanded witness resident for zk_check."""
+ExpCircuit.add_event, evm_circuit/typing.py:880-994; public_data2witness, pi_circuit.py:839-1073).  The functions here
+hand the device the compact data those loops start from — raw code bytes, 15 operation cells, copy events + the copied
+bytes, (base, exponent, identifier) per exponentiation, the raw public-input stream — and leave the expanded witness
+resident for zk_check."""
 from __future__ import annotations
 
 from typing import Dict, List, Optional, Sequence
@@ -123,3 +124,19 @@ def assign_exp_circuit(ctx: native.Context, triples, max_exp_steps: Optional[int
 
     n_min = 0 if max_exp_steps is None else int(max_exp_steps) * ExpCircuit.OFFSET_INCREMENT
     ctx.assign_exp_circuit(exp_events(list(triples)), n_rows_min=n_min, stream=stream)
+
+
+def assign_pi_circuit(ctx: native.Context, public_data, MAX_TXS: int, MAX_CALLDATA_BYTES: int, MAX_WITHDRAWALS: int,
+                      stream: int = 0):
+    """public_data2witness(public_data, MAX_TXS, MAX_CALLDATA_BYTES, MAX_WITHDRAWALS) as one device call from the raw
+    public-input stream, under the module's challenges (pi_circuit.keccak_rand, byte_pow_base, as check_matrices sets
+    them): the rows stay resident as ZK_CIRCUIT_PI, the keccak and calldata gas tables as TABLE_KECCAK /
+    TABLE_CALLDATA_GAS.  Returns (circuit_len, PublicInputs)"""
+    from . import pi_circuit as pc
+
+    ctx.set_challenge(native.CHALLENGE_PI_KECCAK, pc.keccak_rand.n)
+    ctx.set_challenge(native.CHALLENGE_PI_BYTE_BASE, pc.byte_pow_base.n)
+    raw = pc.raw_public_inputs(public_data, MAX_TXS, MAX_CALLDATA_BYTES, MAX_WITHDRAWALS)
+    digest = ctx.assign_pi_circuit(MAX_TXS, MAX_CALLDATA_BYTES, MAX_WITHDRAWALS, raw, stream=stream)
+    b = public_data.block
+    return len(raw), pc.PublicInputs(Word(digest), Word(b.hash), Word(b.state_root), Word(public_data.state_root_prev))

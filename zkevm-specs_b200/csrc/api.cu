@@ -908,6 +908,95 @@ extern "C" int zk_assign_exp_circuit(zk_ctx* ctx, uint64_t n_events, const uint6
   return launched(ctx, "k_assign_exp_chain / k_assign_exp_rows", n_launch);
 }
 
+// the two levels of a PI scan over n items (bytes) in 32-byte chunks
+template <class S>
+static int pi_scan(zk_ctx* ctx, const S& s, typename S::T* x, typename S::T* top, cudaStream_t st) {
+  const u64 n_chunks = (s.n + ZK_SEG_CHUNK - 1) / ZK_SEG_CHUNK, n_blocks = (n_chunks + PI_SCAN_BLOCK_CHUNKS - 1) / PI_SCAN_BLOCK_CHUNKS;
+  k_assign_pi_scan<S><<<(unsigned)n_blocks, 256, 0, st>>>(s, x, top);
+  k_assign_pi_scan_top<S><<<1, 256, 0, st>>>(s, n_blocks, top);
+  return launched(ctx, "k_assign_pi_scan / k_assign_pi_scan_top", 2);
+}
+extern "C" int zk_assign_pi_circuit(zk_ctx* ctx, uint64_t max_txs, uint64_t max_calldata_bytes, uint64_t max_withdrawals,
+                                    const uint8_t* raw_public_inputs, uint64_t n_bytes, uint64_t* pi_keccak_out, void* stream) {
+  CK(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  // everything is validated before the resident matrix, the tables or the circuit length are touched
+  const char* why = pi_shape_error(max_txs, max_calldata_bytes, max_withdrawals, n_bytes);
+  if (why) return fail_msg(ctx, why);
+  std::vector<u64> cd_off(max_txs + 1);
+  if ((why = pi_calldata_offsets(max_txs, max_calldata_bytes, raw_public_inputs, cd_off.data()))) return fail_msg(ctx, why);
+  const u64 n = n_bytes, max_cd = max_calldata_bytes, n_inv = std::max<u64>(256, max_txs + 1);
+  const u64 n_kc = (n + ZK_SEG_CHUNK - 1) / ZK_SEG_CHUNK, n_kb = (n_kc + PI_SCAN_BLOCK_CHUNKS - 1) / PI_SCAN_BLOCK_CHUNKS;
+  const u64 n_gc = (max_cd + ZK_SEG_CHUNK - 1) / ZK_SEG_CHUNK, n_gb = (n_gc + PI_SCAN_BLOCK_CHUNKS - 1) / PI_SCAN_BLOCK_CHUNKS;
+  const size_t s_seq = up32(n), s_cd = s_seq + up32(n), s_inv = s_cd + up32((max_txs + 1) * 8), s_kx = s_inv + n_inv * 32;
+  const size_t s_kt = s_kx + n_kc * sizeof(RlcPair), s_gx = s_kt + n_kb * sizeof(RlcPair), s_gt = s_gx + up32(n_gc * 8);
+  const size_t s_dig = s_gt + up32(n_gb * 8 + 8), s_total = s_dig + 64;
+  int rc;
+  if ((rc = ensure_astage(ctx, s_total))) return rc;
+  Matrix& m = ctx->circ[ZK_CIRCUIT_PI];
+  Matrix& kt = ctx->tab[ZK_TABLE_KECCAK];
+  Matrix& gt = ctx->tab[ZK_TABLE_CALLDATA_GAS];
+  // new versions: indexes cached on the old tables are rebuilt
+  if ((rc = alloc_narrow(ctx, m, n, 28, kPiAssignWidths))) return rc;
+  if ((rc = alloc_narrow(ctx, kt, 2, 5, kPiKeccakWidths))) return rc;
+  if ((rc = alloc_narrow(ctx, gt, 1 + cd_off[max_txs], 3, kPiGasWidths))) return rc;
+  if (!ctx->evm_fork_ev) CK(ctx, cudaEventCreateWithFlags(&ctx->evm_fork_ev, cudaEventDisableTiming));
+  if (!ctx->evm_aux) {
+    CK(ctx, cudaStreamCreateWithFlags(&ctx->evm_aux, cudaStreamNonBlocking));
+    CK(ctx, cudaEventCreateWithFlags(&ctx->evm_join_ev, cudaEventDisableTiming));
+  }
+  unsigned char* sg = ctx->astage;
+  CK(ctx, cudaMemcpyAsync(sg, raw_public_inputs, n, cudaMemcpyHostToDevice, st));
+  CK(ctx, cudaMemcpyAsync(sg + s_cd, cd_off.data(), (max_txs + 1) * 8, cudaMemcpyHostToDevice, st));
+  PiAssign a;
+  a.F = sg;
+  a.seq = sg + s_seq;
+  a.cd_off = (const u64*)(sg + s_cd);
+  a.inv = (Fr*)(sg + s_inv);
+  a.kx = (RlcPair*)(sg + s_kx);
+  a.ktop = (RlcPair*)(sg + s_kt);
+  a.gx = (u64*)(sg + s_gx);
+  a.gtop = (u64*)(sg + s_gt);
+  a.dig = (u64*)(sg + s_dig);
+  a.n = n, a.max_txs = max_txs, a.max_cd = max_cd, a.max_wd = max_withdrawals, a.n_inv = n_inv;
+  a.rand_mont = fr_to_mont(ctx->chal[ZK_CHALLENGE_PI_KECCAK]);
+  a.base_mont = fr_to_mont(ctx->chal[ZK_CHALLENGE_PI_BYTE_BASE]);
+  a.base = (unsigned char*)m.dev;
+  a.kbase = (unsigned char*)kt.dev;
+  a.gbase = (unsigned char*)gt.dev;
+  for (int c = 0; c < 28; c++) a.off[c] = m.off[c];
+  for (int c = 0; c < 5; c++) a.koff[c] = kt.off[c];
+  for (int c = 0; c < 3; c++) a.goff[c] = gt.off[c];
+  k_assign_pi_seq<<<grid_persistent(ctx, k_assign_pi_seq, 256, n), 256, 0, st>>>(a);
+  k_assign_pi_inv<<<(unsigned)((n_inv + 255) / 256), 256, 0, st>>>(a);
+  if ((rc = launched(ctx, "k_assign_pi_seq / k_assign_pi_inv", 2))) return rc;
+  // the sponge is serial: it runs on the auxiliary stream under the row kernels and joins before the digest is written
+  CK(ctx, cudaEventRecord(ctx->evm_fork_ev, st));
+  CK(ctx, cudaStreamWaitEvent(ctx->evm_aux, ctx->evm_fork_ev, 0));
+  k_assign_pi_sponge<<<1, 32, 0, ctx->evm_aux>>>(a);
+  if ((rc = launched(ctx, "k_assign_pi_sponge"))) return rc;
+  CK(ctx, cudaEventRecord(ctx->evm_join_ev, ctx->evm_aux));
+  if ((rc = pi_scan(ctx, PiKrlcScan{a.seq, n, a.rand_mont}, a.kx, a.ktop, st))) return rc;
+  k_assign_pi_krlc<<<(unsigned)((n_kc + 255) / 256), 256, 0, st>>>(a);
+  if ((rc = launched(ctx, "k_assign_pi_krlc"))) return rc;
+  if (max_cd) {
+    if ((rc = pi_scan(ctx, PiGasScan{a.F + PI_TX0 + PI_SLOT_BYTES * max_txs, max_cd}, a.gx, a.gtop, st))) return rc;
+    k_assign_pi_calldata<<<(unsigned)((n_gc + 255) / 256), 256, 0, st>>>(a);
+    if ((rc = launched(ctx, "k_assign_pi_calldata"))) return rc;
+  }
+  k_assign_pi_rows<<<grid_persistent(ctx, k_assign_pi_rows, 256, n), 256, 0, st>>>(a);
+  if ((rc = launched(ctx, "k_assign_pi_rows"))) return rc;
+  CK(ctx, cudaStreamWaitEvent(st, ctx->evm_join_ev, 0));
+  k_assign_pi_finish<<<1, 32, 0, st>>>(a);
+  if ((rc = launched(ctx, "k_assign_pi_finish"))) return rc;
+  ctx->chal[ZK_PARAM_PI_CIRCUIT_LEN] = fr_u64(n);
+  if (pi_keccak_out) {
+    CK(ctx, cudaMemcpyAsync(pi_keccak_out, a.dig + 4, 32, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaStreamSynchronize(st));
+  }
+  return 0;
+}
+
 extern "C" int64_t zk_resident_rows(zk_ctx* ctx, int circuit_id) {
   if (circuit_id < 0 || circuit_id >= ZK_N_CIRCUITS) return -1;
   return (int64_t)ctx->circ[circuit_id].n_rows;

@@ -6,6 +6,8 @@
 //   CopyCircuit.copy         src/zkevm_specs/evm_circuit/typing.py:1010-1147 copy events + bytes -> 20-cell rows
 //   ExpCircuit.add_event     src/zkevm_specs/evm_circuit/typing.py:880-994  (base, exponent, id) -> 21-cell rows
 //                            + the exp table (Tables._convert_exp_circuit_to_table, table.py:654-671)
+//   public_data2witness      src/zkevm_specs/pi_circuit.py:839-1073  raw public-input bytes -> 28-cell rows, one per byte
+//                            + the keccak table and the calldata gas table its lookups read
 //
 // The two sequential pieces — value_rlc of a contract and rlc_acc of a copy event, both Horner chains
 // acc = acc * r + byte — run as a chunked segmented scan: one thread folds a 32-byte chunk
@@ -15,6 +17,7 @@
 // (fr.cuh:ld_col widths), so a check after an assignment reads 80-150 B per row instead of 384-1,824.
 // Included by api.cu (it uses the context).
 #include "circuit.cuh"
+#include "keccak.cuh"
 #include "words.cuh"
 
 namespace zk {
@@ -462,6 +465,355 @@ ZK_HD void assign_exp_row(const ExpAssign& a, u64 r) {
   }
 }
 
+// ---------------------------------------------------------------- public-inputs circuit
+// public_data2witness (pi_circuit.py:839-1073) from the raw public-input stream F = b"".join(rpi_byte_values): one row
+// per byte.  The values (block fields, tx-table fields, calldata bytes, withdrawal fields) lie back to back in F at
+// offsets that are a closed form of MAX_TXS, MAX_CALLDATA_BYTES and MAX_WITHDRAWALS (pi_value_of).  Row r lies in the
+// value whose forward range [s, s + len) holds r and carries F[2s + len - 1 - r]: each value's bytes reversed.  The
+// reference processes the values from last to first, each value's bytes first to last; that order `seq` is row n-1
+// down to row 0, and the digest is keccak256(seq).  rpi_bytes_keccakrlc is one Horner chain over all of seq: chunks of
+// 32 bytes fold to (value, r^32) pairs (rlc_chunk), the pairs are scanned in two levels (a block of 256 threads over 4
+// chunks each, then one block over the block totals), and each chunk replays its bytes from its carried-in value.  The
+// per-tx calldata gas sums use the same scan over integers.  Everything else of a row is a closed form of the row and
+// the few bytes it names.
+#define PI_BLOCK_BYTES 8437ull  // N_BYTES_ONE + N_BYTES_BLOCK + N_BYTES_EXTRA_VALUE: the block section + 3 Words
+#define PI_TX0 8454ull          // the first tx slot, after the empty tx row's (tx_id 8, index 8, value 1)
+#define PI_SLOT_BYTES 336ull    // one tx slot: 10 fields of (tx_id 8, index 8, value lo, [value hi 16])
+#define PI_WD_BYTES 56ull       // one withdrawal: id 8, validator_id 8, address lo 16, hi 16, amount 8
+#define PI_CDL_OFF 256ull       // the CallDataLength value inside a slot (field 7's lo)
+#define PI_TX_LEN 10ull
+#define PI_TAG_CALLDATA 13  // TxContextFieldTag.CallData
+#define PI_CDL_TAG 8        // TxContextFieldTag.CallDataLength
+#define PI_SCAN_GROUP 4               // chunks per thread of k_assign_pi_scan
+#define PI_SCAN_BLOCK_CHUNKS 1024ull  // chunks per block of k_assign_pi_scan (256 threads)
+// the 28 cells of ZK_CIRCUIT_PI (pi.cu P_*), and the narrow width of each: flags, bytes and tags 1 B, counters and ids
+// 8 B, Word halves 16 B, accumulators, inverses and the tx value lo (a 160-bit address is a Value) 32 B
+enum { PA_QLAST, PA_QTX, PA_QCD, PA_QCD_START, PA_QKECCAK, PA_QVSTART, PA_TXID_INV, PA_VLO_INV, PA_DIFF_INV, PA_GAS,
+       PA_FINAL, PA_QWD, PA_BYTES, PA_KRLC, PA_VLC, PA_DIG_LO, PA_DIG_HI, PA_QEN, PA_TXID, PA_TAG, PA_INDEX, PA_VLO, PA_VHI,
+       PA_WD_ID, PA_WD_VAL, PA_WD_ALO, PA_WD_AHI, PA_WD_AMT };
+static const unsigned char kPiAssignWidths[28] = {1, 1, 1, 1, 1, 1, 32, 32, 32, 8, 1, 1, 1, 32,
+                                                  32, 16, 16, 1, 8, 1, 8, 32, 16, 8, 8, 16, 16, 8};
+static const unsigned char kPiKeccakWidths[5] = {1, 32, 8, 16, 16};  // is_enabled, input_rlc, input_len, output lo, hi
+static const unsigned char kPiGasWidths[3] = {8, 1, 8};              // tx_id, is_final, gas_cost_acc
+
+struct RlcPair {
+  Fr v, p;  // Horner value (canonical), r^len (Montgomery form)
+};
+ZK_HD RlcPair rlc_pair_op(const RlcPair& l, const RlcPair& r) {
+  RlcPair o = l;
+  rlc_combine(o.v, o.p, r.v, r.p);
+  return o;
+}
+// the two scans: fold(lo, hi) is the monoid value of items [lo, hi), op combines left and right
+struct PiKrlcScan {
+  typedef RlcPair T;
+  const unsigned char* seq;
+  u64 n;
+  Fr r_mont;
+  ZK_HD T id() const { return RlcPair{fr_u64(0), fr_to_mont(fr_u64(1))}; }
+  ZK_HD T fold(u64 lo, u64 hi) const {
+    RlcPair o;
+    rlc_chunk(seq, lo, hi, r_mont, o.v, o.p);
+    return o;
+  }
+  static ZK_HD T op(const T& l, const T& r) { return rlc_pair_op(l, r); }
+};
+ZK_HD u64 pi_cd_cost(u64 b) { return b ? 16 : 4; }  // GAS_COST_TX_CALL_DATA_PER_(NON_)ZERO_BYTE
+struct PiGasScan {
+  typedef u64 T;
+  const unsigned char* cd;  // the calldata bytes
+  u64 n;
+  ZK_HD T id() const { return 0; }
+  ZK_HD T fold(u64 lo, u64 hi) const {
+    u64 g = 0;
+    for (u64 j = lo; j < hi; j++) g += pi_cd_cost(cd[j]);
+    return g;
+  }
+  static ZK_HD T op(const T& l, const T& r) { return l + r; }
+};
+
+struct PiAssign {
+  const unsigned char* F;  // the forward stream, n bytes
+  unsigned char* seq;      // processing order: seq[n - 1 - r] = the byte of row r
+  const u64* cd_off;       // [max_txs + 1] prefix sums of the CallDataLength fields
+  Fr* inv;                 // [n_inv] 1/k (inv[0] = 0), n_inv = max(256, max_txs + 1)
+  RlcPair* kx;             // per 32-byte chunk of seq: the Horner pair carried in from its block's earlier chunks
+  RlcPair* ktop;           // per block of PI_SCAN_BLOCK_CHUNKS chunks: the pair carried in from earlier blocks
+  u64* gx;                 // the same two arrays of the calldata gas scan
+  u64* gtop;
+  u64* dig;                // [4] keccak256(seq) as little-endian lanes, then [4] the digest Word (lo 2 limbs, hi 2 limbs)
+  u64 n, max_txs, max_cd, max_wd, n_inv;
+  Fr rand_mont, base_mont;  // ZK_CHALLENGE_PI_KECCAK, ZK_CHALLENGE_PI_BYTE_BASE in Montgomery form
+  unsigned char* base;      // the circuit's narrow columns
+  u64 off[28];
+  unsigned char* kbase;  // the keccak table: 2 rows
+  u64 koff[5];
+  unsigned char* gbase;  // the calldata gas table: the zero row + one row per used calldata byte
+  u64 goff[3];
+};
+
+// tx field f of a slot: its value lo is 20 bytes (from, to: 160-bit Values), 16 (Word lo) or 8; Words add a 16-byte hi
+ZK_HD bool pi_field_word(u64 f) { return f == 2 || f == 6 || f == 9; }
+ZK_HD u64 pi_field_lo(u64 f) { return (f == 3 || f == 4) ? 20 : pi_field_word(f) ? 16 : 8; }
+ZK_HD u64 pi_field_len(u64 f) { return 16 + pi_field_lo(f) + (pi_field_word(f) ? 16 : 0); }
+ZK_HD u64 pi_field_off(u64 f) {
+  u64 o = 0;
+  for (u64 g = 0; g < f; g++) o += pi_field_len(g);
+  return o;
+}
+// the first ten values of the block section (0, coinbase, gas_limit, number, time, prev_randao lo, hi, base_fee lo, hi,
+// chain_id); 16-byte Word halves follow from byte 117
+ZK_HD u64 pi_head_len(u64 i) { return i == 0 ? 1 : i == 1 ? 20 : (i >= 5 && i <= 8) ? 16 : 8; }
+
+// the value [s, s + len) of the forward stream that holds byte r
+ZK_HD void pi_value_of(const PiAssign& a, u64 r, u64& s, u64& len) {
+  const u64 c0 = PI_TX0 + PI_SLOT_BYTES * a.max_txs, w0 = c0 + a.max_cd;
+  if (r < 117) {
+    u64 o = 0, i = 0;
+    while (o + pi_head_len(i) <= r) o += pi_head_len(i++);
+    s = o, len = pi_head_len(i);
+  } else if (r < PI_BLOCK_BYTES) {
+    s = r - (r - 117) % 16, len = 16;
+  } else if (r < PI_TX0) {  // the empty tx row: tx_id 8, index 8, value 1
+    s = r < PI_BLOCK_BYTES + 8 ? PI_BLOCK_BYTES : r < PI_BLOCK_BYTES + 16 ? PI_BLOCK_BYTES + 8 : PI_BLOCK_BYTES + 16;
+    len = r < PI_BLOCK_BYTES + 16 ? 8 : 1;
+  } else if (r < c0) {
+    u64 b = r - (r - PI_TX0) % PI_SLOT_BYTES, f = 0;
+    while (b + pi_field_len(f) <= r) b += pi_field_len(f++);
+    const u64 q = r - b, lo = pi_field_lo(f);
+    if (q < 16) s = b + (q & 8), len = 8;  // tx_id, index
+    else if (q < 16 + lo) s = b + 16, len = lo;
+    else s = b + 16 + lo, len = 16;
+  } else if (r < w0) {
+    s = r, len = 1;
+  } else {
+    const u64 o = (r - w0) % PI_WD_BYTES, b = r - o;
+    if (o < 16) s = b + (o & 8), len = 8;
+    else if (o < 48) s = b + (o & ~15ull), len = 16;  // address lo, hi
+    else s = b + 48, len = 8;
+  }
+}
+ZK_HD u64 pi_byte(const PiAssign& a, u64 r) {
+  u64 s, len;
+  pi_value_of(a, r, s, len);
+  return a.F[2 * s + len - 1 - r];
+}
+// nb <= 20 big-endian bytes as an integer (< 2^160)
+ZK_HD Fr pi_be(const unsigned char* p, u64 nb) {
+  u64 l0 = 0, l1 = 0, l2 = 0;
+  for (u64 i = 0; i < nb; i++) {
+    const u64 k = nb - 1 - i, v = (u64)p[i] << (8 * (k & 7));
+    if (k < 8) l0 |= v;
+    else if (k < 16) l1 |= v;
+    else l2 |= v;
+  }
+  return Fr{{l0, l1, l2, 0}};
+}
+// 1/k for |k| < n_inv, from the staged table
+ZK_HD Fr pi_inv_small(const PiAssign& a, u64 k, bool neg) {
+  const Fr v = a.inv[k];
+  return neg ? fr_sub(fr_u64(0), v) : v;
+}
+// the largest slot j < max_txs with cd_off[j] <= k: the tx whose calldata holds byte k (when k < cd_off[max_txs])
+ZK_HD u64 pi_slot_of(const PiAssign& a, u64 k) {
+  u64 lo = 0, hi = a.max_txs;
+  while (hi - lo > 1) {
+    const u64 mid = (lo + hi) >> 1;
+    if (a.cd_off[mid] <= k) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+// the gas of calldata bytes [0, x), x < max_cd, from the scan
+ZK_HD u64 pi_gas_before(const PiAssign& a, u64 x) {
+  const u64 c = x / ZK_SEG_CHUNK, c0 = PI_TX0 + PI_SLOT_BYTES * a.max_txs;
+  u64 g = a.gtop[c / PI_SCAN_BLOCK_CHUNKS] + a.gx[c];
+  for (u64 j = c * ZK_SEG_CHUNK; j < x; j++) g += pi_cd_cost(a.F[c0 + j]);
+  return g;
+}
+
+ZK_HD void assign_pi_seq(const PiAssign& a, u64 r) { a.seq[a.n - 1 - r] = (unsigned char)pi_byte(a, r); }
+ZK_HD void assign_pi_inv(const PiAssign& a, u64 k) { a.inv[k] = fr_inv(fr_u64(k)); }
+
+// rpi_bytes_keccakrlc of the rows of 32-byte chunk c of seq (rows n-1-t for t in the chunk), from its carried-in value
+ZK_HD void assign_pi_krlc(const PiAssign& a, u64 c) {
+  const u64 t0 = c * ZK_SEG_CHUNK, t1 = zk_min64(t0 + ZK_SEG_CHUNK, a.n);
+  Fr acc = rlc_pair_op(a.ktop[c / PI_SCAN_BLOCK_CHUNKS], a.kx[c]).v;
+  for (u64 t = t0; t < t1; t++) {
+    acc = fr_add_u64(fr_montmul(acc, a.rand_mont), a.seq[t]);
+    st_fr(a.base + a.off[PA_KRLC], a.n - 1 - t, acc);
+  }
+}
+
+// the tx-table cells of the calldata rows 10 * max_txs + 1 + k for the bytes k of 32-byte chunk c of the calldata, and
+// their gas-table rows 1 + k.  Byte k belongs to the tx slot j with cd_off[j] <= k < cd_off[j + 1]; bytes from
+// cd_off[max_txs] on are padding (tx_id, index, gas, is_final all 0), whose gas row would repeat the zero row: the table
+// holds the zero row and the used bytes' rows only, the reference's set without copies.  (A lookup counts identical rows
+// once by walking them, so ~n copies of the zero row cost each lookup of it ~n probes.)
+ZK_HD void assign_pi_calldata(const PiAssign& a, u64 c) {
+  const u64 k0 = c * ZK_SEG_CHUNK, k1 = zk_min64(k0 + ZK_SEG_CHUNK, a.max_cd), total = a.cd_off[a.max_txs];
+  const u64 row0 = PI_TX_LEN * a.max_txs + 1, c0 = PI_TX0 + PI_SLOT_BYTES * a.max_txs;
+  u64 j = pi_slot_of(a, k0);
+  u64 g = k0 < total ? pi_gas_before(a, k0) - pi_gas_before(a, a.cd_off[j]) : 0;  // gas of this tx's bytes before k0
+  unsigned char* B = a.base;
+  unsigned char* T = a.gbase;
+  for (u64 k = k0; k < k1; k++) {
+    while (j + 1 < a.max_txs && a.cd_off[j + 1] <= k) j++, g = 0;  // a new tx starts at k
+    const u64 b = a.F[c0 + k];
+    const bool used = k < total;
+    g += pi_cd_cost(b);
+    const u64 tx_id = used ? j + 1 : 0, idx = used ? k - a.cd_off[j] : 0, gas = used ? g : 0;
+    const bool fin = used && k + 1 == a.cd_off[j + 1];
+    u64 nxt = 0;  // the next row's tx_id (0 after the last calldata row)
+    if (k + 1 < total) {
+      u64 jn = j;
+      while (jn + 1 < a.max_txs && a.cd_off[jn + 1] <= k + 1) jn++;
+      nxt = jn + 1;
+    }
+    const u64 r = row0 + k;
+    B[a.off[PA_QTX] + r] = 0;
+    B[a.off[PA_QCD] + r] = 1;
+    B[a.off[PA_QCD_START] + r] = k == 0;
+    st_fr(B + a.off[PA_TXID_INV], r, a.inv[tx_id]);
+    st_fr(B + a.off[PA_VLO_INV], r, a.inv[b]);
+    st_fr(B + a.off[PA_DIFF_INV], r, nxt >= tx_id ? pi_inv_small(a, nxt - tx_id, false) : pi_inv_small(a, tx_id - nxt, true));
+    ((u64*)(B + a.off[PA_GAS]))[r] = gas;
+    B[a.off[PA_FINAL] + r] = fin;
+    ((u64*)(B + a.off[PA_TXID]))[r] = tx_id;
+    B[a.off[PA_TAG] + r] = PI_TAG_CALLDATA;
+    ((u64*)(B + a.off[PA_INDEX]))[r] = idx;
+    st_fr(B + a.off[PA_VLO], r, fr_u64(b));
+    st_u128(B + a.off[PA_VHI], r, 0, 0);
+    if (used) {
+      ((u64*)(T + a.goff[0]))[1 + k] = tx_id;
+      T[a.goff[1] + 1 + k] = fin;
+      ((u64*)(T + a.goff[2]))[1 + k] = gas;
+    }
+  }
+}
+
+// every cell of row r but rpi_bytes_keccakrlc, the calldata rows' tx-table cells and row 0's digest
+ZK_HD void assign_pi_row(const PiAssign& a, u64 r) {
+  unsigned char* B = a.base;
+  const unsigned char* F = a.F;
+  u64 s, len;
+  pi_value_of(a, r, s, len);
+  const u64 last = 2 * s + len - 1 - r;  // the forward position of this row's byte
+  Fr lc = fr_u64(0);  // rpi_value_lc: Horner over the value's bytes from its first one to this row's
+  for (u64 j = s; j <= last; j++) lc = fr_add_u64(fr_montmul(lc, a.base_mont), F[j]);
+  B[a.off[PA_QLAST] + r] = r == a.n - 1;
+  B[a.off[PA_QKECCAK] + r] = r == 0;
+  B[a.off[PA_QVSTART] + r] = r == s + len - 1;
+  B[a.off[PA_BYTES] + r] = F[last];
+  st_fr(B + a.off[PA_VLC], r, lc);
+  st_u128(B + a.off[PA_DIG_LO], r, 0, 0);
+  st_u128(B + a.off[PA_DIG_HI], r, 0, 0);
+  B[a.off[PA_QEN] + r] = 1;
+  const u64 n_tx = PI_TX_LEN * a.max_txs + 1, n_cd = n_tx + a.max_cd;
+  if (r < n_tx || r >= n_cd) {  // a tx-table row (the empty row 0, then slot (r - 1) / 10, field (r - 1) % 10), or none
+    u64 tx_id = 0, idx = 0, tag = 0, h0 = 0, h1 = 0;
+    Fr lo = fr_u64(0), tag_inv = fr_u64(0), lo_inv = fr_u64(0);
+    if (r < n_tx) {
+      u64 b = PI_BLOCK_BYTES, w = 1;
+      bool word = false;
+      if (r) {
+        const u64 f = (r - 1) % PI_TX_LEN;
+        b = PI_TX0 + PI_SLOT_BYTES * ((r - 1) / PI_TX_LEN) + pi_field_off(f);
+        w = pi_field_lo(f);
+        word = pi_field_word(f);
+        tag = f + 1;  // i % TX_LEN or TX_LEN
+      }
+      tx_id = pi_be(F + b, 8).l[0];
+      idx = pi_be(F + b + 8, 8).l[0];
+      lo = pi_be(F + b + 16, w);
+      if (word) {
+        const Fr h = pi_be(F + b + 16 + w, 16);
+        h0 = h.l[0], h1 = h.l[1];
+      }
+      tag_inv = tag >= PI_CDL_TAG ? pi_inv_small(a, tag - PI_CDL_TAG, false) : pi_inv_small(a, PI_CDL_TAG - tag, true);
+      lo_inv = fr_inv(lo);
+    }
+    B[a.off[PA_QTX] + r] = r < n_tx;
+    B[a.off[PA_QCD] + r] = 0;
+    B[a.off[PA_QCD_START] + r] = 0;
+    st_fr(B + a.off[PA_TXID_INV], r, tag_inv);
+    st_fr(B + a.off[PA_VLO_INV], r, lo_inv);
+    st_fr(B + a.off[PA_DIFF_INV], r, fr_u64(0));
+    ((u64*)(B + a.off[PA_GAS]))[r] = 0;
+    B[a.off[PA_FINAL] + r] = 0;
+    ((u64*)(B + a.off[PA_TXID]))[r] = tx_id;
+    B[a.off[PA_TAG] + r] = (unsigned char)tag;
+    ((u64*)(B + a.off[PA_INDEX]))[r] = idx;
+    st_fr(B + a.off[PA_VLO], r, lo);
+    st_u128(B + a.off[PA_VHI], r, h0, h1);
+  }
+  u64 wd[7] = {0, 0, 0, 0, 0, 0, 0};  // id, validator_id, address lo (2 limbs), hi (2 limbs), amount
+  const bool is_wd = r >= n_cd && r - n_cd < a.max_wd;
+  if (is_wd) {
+    const unsigned char* p = F + PI_TX0 + PI_SLOT_BYTES * a.max_txs + a.max_cd + PI_WD_BYTES * (r - n_cd);
+    const Fr lo = pi_be(p + 16, 16), hi = pi_be(p + 32, 16);
+    wd[0] = pi_be(p, 8).l[0], wd[1] = pi_be(p + 8, 8).l[0], wd[2] = lo.l[0], wd[3] = lo.l[1], wd[4] = hi.l[0], wd[5] = hi.l[1];
+    wd[6] = pi_be(p + 48, 8).l[0];
+  }
+  B[a.off[PA_QWD] + r] = is_wd;
+  ((u64*)(B + a.off[PA_WD_ID]))[r] = wd[0];
+  ((u64*)(B + a.off[PA_WD_VAL]))[r] = wd[1];
+  st_u128(B + a.off[PA_WD_ALO], r, wd[2], wd[3]);
+  st_u128(B + a.off[PA_WD_AHI], r, wd[4], wd[5]);
+  ((u64*)(B + a.off[PA_WD_AMT]))[r] = wd[6];
+  if (r == 0) {  // the gas table's zero row
+    unsigned char* T = a.gbase;
+    ((u64*)(T + a.goff[0]))[0] = 0;
+    T[a.goff[1]] = 0;
+    ((u64*)(T + a.goff[2]))[0] = 0;
+  }
+}
+
+// after the sponge and the keccak RLC: row 0's digest cells, the keccak table (0, 0, 0, 0, 0), (1, krlc[0], n, digest
+// lo, hi), and the digest Word at dig[4..8].  The reference's Word(keccak256(seq)) reads the 32 digest bytes
+// little-endian (lo = bytes 0..15), so its limbs are the sponge's first four lanes as they are.
+ZK_HD void assign_pi_finish(const PiAssign& a) {
+  const u64 lo[2] = {a.dig[0], a.dig[1]}, hi[2] = {a.dig[2], a.dig[3]};
+  unsigned char* B = a.base;
+  st_u128(B + a.off[PA_DIG_LO], 0, lo[0], lo[1]);
+  st_u128(B + a.off[PA_DIG_HI], 0, hi[0], hi[1]);
+  unsigned char* K = a.kbase;
+  const Fr rlc = ld_col(B + a.off[PA_KRLC], 32, 0);
+  K[a.koff[0]] = 0;
+  K[a.koff[0] + 1] = 1;
+  st_fr(K + a.koff[1], 0, fr_u64(0));
+  st_fr(K + a.koff[1], 1, rlc);
+  ((u64*)(K + a.koff[2]))[0] = 0;
+  ((u64*)(K + a.koff[2]))[1] = a.n;
+  st_u128(K + a.koff[3], 0, 0, 0);
+  st_u128(K + a.koff[3], 1, lo[0], lo[1]);
+  st_u128(K + a.koff[4], 0, 0, 0);
+  st_u128(K + a.koff[4], 1, hi[0], hi[1]);
+  a.dig[4] = lo[0], a.dig[5] = lo[1], a.dig[6] = hi[0], a.dig[7] = hi[1];
+}
+
+// host validation of zk_assign_pi_circuit (and of the CPU emulation): nullptr if the stream's length, the maxima and
+// the CallDataLength fields are acceptable, with cd_off[max_txs + 1] filled; the reason otherwise
+static const char* pi_shape_error(u64 max_txs, u64 max_cd, u64 max_wd, u64 n_bytes) {
+  if (max_txs == 0) return "public inputs: MAX_TXS must be at least 1 (the reference asserts a tx)";
+  if (max_wd == 0) return "public inputs: MAX_WITHDRAWALS must be at least 1 (the reference asserts a withdrawal)";
+  if (max_txs >= (1ull << 31) || max_cd >= (1ull << 31) || max_wd >= (1ull << 31))
+    return "public inputs: too many rows (row ids are below 2^31 - 1)";
+  if (n_bytes != PI_TX0 + PI_SLOT_BYTES * max_txs + max_cd + PI_WD_BYTES * max_wd)
+    return "public inputs: the stream's length is not the circuit_len of the three maxima";
+  if (n_bytes >= 0x7FFFFFFFull) return "public inputs: too many rows (row ids are below 2^31 - 1)";
+  return nullptr;
+}
+static const char* pi_calldata_offsets(u64 max_txs, u64 max_cd, const unsigned char* raw, u64* cd_off) {
+  cd_off[0] = 0;
+  for (u64 j = 0; j < max_txs; j++) {
+    const u64 len = pi_be(raw + PI_TX0 + PI_SLOT_BYTES * j + PI_CDL_OFF, 8).l[0];
+    if (len > max_cd - cd_off[j]) return "public inputs: the CallDataLength fields sum to more than MAX_CALLDATA_BYTES";
+    cd_off[j + 1] = cd_off[j] + len;
+  }
+  return nullptr;
+}
+
 #ifdef __CUDACC__
 __global__ void __launch_bounds__(256) k_seg_local(SegHorner s, Fr* chunk_val) {
   const u64 c = (u64)blockIdx.x * blockDim.x + threadIdx.x;
@@ -495,6 +847,79 @@ __global__ void __launch_bounds__(128) k_assign_exp_chain(const __grid_constant_
 __global__ void __launch_bounds__(256) k_assign_exp_rows(const __grid_constant__ ExpAssign a) {
   const u64 stride = (u64)gridDim.x * blockDim.x;
   for (u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x; r < a.n_rows; r += stride) assign_exp_row(a, r);
+}
+
+// ---- public-inputs circuit
+__global__ void __launch_bounds__(256) k_assign_pi_seq(const __grid_constant__ PiAssign a) {
+  const u64 stride = (u64)gridDim.x * blockDim.x;
+  for (u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x; r < a.n; r += stride) assign_pi_seq(a, r);
+}
+__global__ void __launch_bounds__(256) k_assign_pi_inv(const __grid_constant__ PiAssign a) {
+  const u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < a.n_inv) assign_pi_inv(a, k);
+}
+// the digest: one thread runs the sponge over all of seq (about n / 136 permutations)
+__global__ void __launch_bounds__(32) k_assign_pi_sponge(const __grid_constant__ PiAssign a) {
+  if (threadIdx.x == 0) keccak256(a.seq, a.n, a.dig);
+}
+// exclusive scan of the values of a block (Hillis-Steele in shared memory); sh[blockDim.x - 1] is left holding the
+// block's combined value
+template <class S>
+__device__ __forceinline__ typename S::T pi_block_excl(const S& s, typename S::T x, typename S::T* sh) {
+  sh[threadIdx.x] = x;
+  __syncthreads();
+  for (u32 d = 1; d < blockDim.x; d <<= 1) {
+    const typename S::T y = threadIdx.x >= d ? S::op(sh[threadIdx.x - d], sh[threadIdx.x]) : sh[threadIdx.x];
+    __syncthreads();
+    sh[threadIdx.x] = y;
+    __syncthreads();
+  }
+  return threadIdx.x ? sh[threadIdx.x - 1] : s.id();
+}
+// level 1: each thread folds PI_SCAN_GROUP 32-byte chunks; x[c] = the value carried into chunk c from the earlier chunks
+// of its block, top[b] = block b's total
+template <class S>
+__global__ void __launch_bounds__(256) k_assign_pi_scan(const __grid_constant__ S s, typename S::T* x, typename S::T* top) {
+  __shared__ typename S::T sh[256];
+  const u64 n_chunks = (s.n + ZK_SEG_CHUNK - 1) / ZK_SEG_CHUNK;
+  const u64 c0 = ((u64)blockIdx.x * blockDim.x + threadIdx.x) * PI_SCAN_GROUP;
+  const typename S::T v = c0 < n_chunks ? s.fold(c0 * ZK_SEG_CHUNK, zk_min64((c0 + PI_SCAN_GROUP) * ZK_SEG_CHUNK, s.n)) : s.id();
+  typename S::T carry = pi_block_excl(s, v, sh);
+  if (threadIdx.x == 0) top[blockIdx.x] = sh[blockDim.x - 1];
+  for (u64 c = c0; c < c0 + PI_SCAN_GROUP && c < n_chunks; c++) {
+    x[c] = carry;
+    carry = S::op(carry, s.fold(c * ZK_SEG_CHUNK, zk_min64((c + 1) * ZK_SEG_CHUNK, s.n)));
+  }
+}
+// level 2, one block: top[b] becomes the value carried into block b (each thread walks a contiguous run of totals)
+template <class S>
+__global__ void __launch_bounds__(256) k_assign_pi_scan_top(const __grid_constant__ S s, u64 n_blocks, typename S::T* top) {
+  __shared__ typename S::T sh[256];
+  const u64 per = (n_blocks + blockDim.x - 1) / blockDim.x;
+  const u64 b0 = zk_min64(threadIdx.x * per, n_blocks), b1 = zk_min64(b0 + per, n_blocks);
+  typename S::T v = s.id();
+  for (u64 b = b0; b < b1; b++) v = S::op(v, top[b]);
+  typename S::T carry = pi_block_excl(s, v, sh);
+  for (u64 b = b0; b < b1; b++) {
+    const typename S::T t = top[b];
+    top[b] = carry;
+    carry = S::op(carry, t);
+  }
+}
+__global__ void __launch_bounds__(256) k_assign_pi_krlc(const __grid_constant__ PiAssign a) {
+  const u64 c = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c < (a.n + ZK_SEG_CHUNK - 1) / ZK_SEG_CHUNK) assign_pi_krlc(a, c);
+}
+__global__ void __launch_bounds__(256) k_assign_pi_calldata(const __grid_constant__ PiAssign a) {
+  const u64 c = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c < (a.max_cd + ZK_SEG_CHUNK - 1) / ZK_SEG_CHUNK) assign_pi_calldata(a, c);
+}
+__global__ void __launch_bounds__(256) k_assign_pi_rows(const __grid_constant__ PiAssign a) {
+  const u64 stride = (u64)gridDim.x * blockDim.x;
+  for (u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x; r < a.n; r += stride) assign_pi_row(a, r);
+}
+__global__ void __launch_bounds__(32) k_assign_pi_finish(const __grid_constant__ PiAssign a) {
+  if (threadIdx.x == 0) assign_pi_finish(a);
 }
 #endif
 

@@ -357,6 +357,22 @@ __host__ __device__ __forceinline__ Fr fr_to_mont(const Fr& a) {
 __host__ __device__ __forceinline__ Fr fr_mul(const Fr& a, const Fr& b) {
   return fr_montmul(fr_to_mont(a), b);
 }
+// a^-1 mod p by Fermat, a^(p-2), over fr_montmul (canonical in and out); fr_inv(0) = 0, the reference's convention for
+// the inverse witnesses.  ~380 products: the row builders call it only where the operand is not a small integer.
+__host__ __device__ __forceinline__ Fr fr_inv(const Fr& a) {
+  const Fr am = fr_to_mont(a);
+  Fr x = fr_to_mont(fr_u64(1));
+#pragma unroll
+  for (int k = 3; k >= 0; k--) {  // the limbs of p - 2, picked by comparison (no run-time index into a local array)
+    const u64 e = k == 3 ? ZK_P3 : k == 2 ? ZK_P2 : k == 1 ? ZK_P1 : ZK_P0 - 2;
+#pragma unroll 1
+    for (int b = 63; b >= 0; b--) {
+      x = fr_montmul(x, x);
+      if ((e >> b) & 1) x = fr_montmul(x, am);
+    }
+  }
+  return fr_montmul(x, fr_u64(1));  // out of Montgomery form
+}
 // a (canonical, fits 64 bits) times small constant-free u64, exact integer if it fits,
 // else mod p: used for cheap "x * 256^k"-style terms
 __host__ __device__ __forceinline__ Fr fr_shl_small(u64 v, int bits) {  // v * 2^bits, bits<192, as integer (< p guaranteed by caller)

@@ -76,7 +76,7 @@ EXPORTS = [
     "zk_upload_bytecode_table_from_code", "zk_nccl_unique_id", "zk_nccl_comm_init", "zk_nccl_comm_destroy",
     "zk_keccak256_batch", "zk_assign_keccak_table", "zk_assign_bytecode_circuit", "zk_assign_state_circuit",
     "zk_assign_copy_circuit", "zk_download_columns", "zk_resident_rows", "zk_assign_exp_circuit", "zk_table_rows",
-    "zk_download_table",
+    "zk_download_table", "zk_assign_pi_circuit",
 ]
 
 
@@ -122,6 +122,7 @@ def lib() -> ctypes.CDLL:
         L.zk_table_rows.argtypes = [vp, i32]
         L.zk_table_rows.restype = ctypes.c_int64
         L.zk_download_table.argtypes = [vp, i32, vp, vp]
+        L.zk_assign_pi_circuit.argtypes = [vp, u64, u64, u64, vp, u64, vp, vp]
         L.zk_circuit_cols.argtypes = [i32]
         L.zk_table_cols.argtypes = [i32]
         L.zk_n_constraints.argtypes = [i32]
@@ -300,6 +301,22 @@ class Context:
         ev = np.ascontiguousarray(events, dtype=np.uint64).reshape(-1, 12)
         self._ck(self._L.zk_assign_exp_circuit(self._h, ev.shape[0], _host_ptr(ev), int(n_rows_min), ctypes.c_void_p(stream)),
                  "zk_assign_exp_circuit")
+
+    def assign_pi_circuit(self, max_txs: int, max_calldata_bytes: int, max_withdrawals: int, raw, digest: bool = True,
+                          stream: int = 0) -> Optional[int]:
+        """public_data2witness (pi_circuit.py:839-1073) on the device from the raw public-input stream (bytes or uint8,
+        pi_circuit.raw_public_inputs): the rows stay resident as ZK_CIRCUIT_PI, the keccak and calldata gas tables they
+        look up REPLACE the resident TABLE_KECCAK and TABLE_CALLDATA_GAS, PARAM_PI_CIRCUIT_LEN becomes the row count;
+        the challenges CHALLENGE_PI_KECCAK / CHALLENGE_PI_BYTE_BASE are read from the context.  digest=True waits for
+        the call and returns keccak256 of the bytes in processing order as an int (the pi_keccak Word)"""
+        buf = np.frombuffer(bytes(raw), dtype=np.uint8) if not isinstance(raw, np.ndarray) else np.ascontiguousarray(raw, dtype=np.uint8)
+        out = np.zeros(4, dtype=np.uint64)
+        self._ck(self._L.zk_assign_pi_circuit(self._h, int(max_txs), int(max_calldata_bytes), int(max_withdrawals),
+                                              _host_ptr(buf), buf.shape[0], _host_ptr(out) if digest else None,
+                                              ctypes.c_void_p(stream)), "zk_assign_pi_circuit")
+        if not digest:
+            return None
+        return sum(int(x) << (64 * i) for i, x in enumerate(out))
 
     def download_columns(self, circuit_id: int, stream: int = 0):
         """the resident matrix of a circuit as canonical cells + its row flags: (uint64[n_cols][n_rows][4], uint8[n_rows])"""

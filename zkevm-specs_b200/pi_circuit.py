@@ -106,8 +106,9 @@ class Transaction:
                 _value(1 if self.to_addr is None else 0), _word(self.value), _value(len(self.data)),
                 _value(self.call_data_gas_cost()), _word(self.tx_sign_hash)]
 
-    def tx_raw_bytes(self, tx_id: int) -> List[bytes]:
-        """(tx_id, index = 0, value lo, [value hi]) big-endian per field (:524-583)"""
+    def tx_raw_bytes(self, tx_id: int, call_data_gas_cost: Optional[int] = None) -> List[bytes]:
+        """(tx_id, index = 0, value lo, [value hi]) big-endian per field (:524-583); `call_data_gas_cost` saves the
+        per-byte sum when the caller has it"""
         out: List[bytes] = []
 
         def put(lo: bytes, hi: bytes = b""):
@@ -129,7 +130,8 @@ class Transaction:
         put((1 if self.to_addr is None else 0).to_bytes(8, "big"))
         put_word(self.value)
         put(len(self.data).to_bytes(8, "big"))
-        put(self.call_data_gas_cost().to_bytes(8, "big"))
+        gas = self.call_data_gas_cost() if call_data_gas_cost is None else call_data_gas_cost
+        put(int(gas).to_bytes(8, "big"))
         put_word(self.tx_sign_hash)
         return out
 
@@ -476,6 +478,29 @@ def public_data2witness(public_data: PublicData, MAX_TXS: int, MAX_CALLDATA_BYTE
                    copy_constrains=values)
 
 
+def raw_public_inputs(public_data: PublicData, MAX_TXS: int, MAX_CALLDATA_BYTES: int, MAX_WITHDRAWALS: int) -> bytes:
+    """the raw public-input stream b"".join(public_data2witness(...).copy_constrains) (pi_circuit.py:845-856), built
+    without a Python object per calldata byte: what zk_assign_pi_circuit expands on the device"""
+    pd = public_data
+    values: List[bytes] = list(pd.block_table_raw_byte_values())
+    for v in (pd.block.hash, pd.block.state_root, pd.state_root_prev):
+        lo, hi = _lo_hi(v)
+        values += [lo.to_bytes(16, "big"), hi.to_bytes(16, "big")]
+    assert len(pd.txs) > 0
+    values += [(0).to_bytes(8, "big"), (0).to_bytes(8, "big"), (0).to_bytes(1, "big")]  # the empty first tx row
+    data = [np.frombuffer(bytes(tx.data), dtype=np.uint8) for tx in pd.txs]
+    for i, tx in enumerate(pd._txs_padded(MAX_TXS)):
+        d = data[i] if i < len(data) else data[0][:0]
+        gas = GAS_COST_TX_CALL_DATA_PER_ZERO_BYTE * len(d) + (GAS_COST_TX_CALL_DATA_PER_NON_ZERO_BYTE
+                                                               - GAS_COST_TX_CALL_DATA_PER_ZERO_BYTE) * int(np.count_nonzero(d))
+        values += tx.tx_raw_bytes(i + 1, gas)
+    calldata = np.concatenate(data).tobytes()
+    assert len(calldata) <= MAX_CALLDATA_BYTES
+    values += [calldata, bytes(MAX_CALLDATA_BYTES - len(calldata))]
+    values += pd.withdrawal_table_raw_bytes(MAX_WITHDRAWALS)
+    return b"".join(values)
+
+
 # ------------------------------------------------------------------------------------------ verification
 def check_matrices(ctx: native.Context, cells: np.ndarray, keccak: np.ndarray, gas: np.ndarray, circuit_len: int,
                    row_begin: int = 0, row_end: Optional[int] = None, row_base: int = 0, flags: int = native.FLAG_WRAP):
@@ -533,6 +558,22 @@ def _copy_constraints(witness: Witness, MAX_TXS: int, MAX_CALLDATA_BYTES: int, M
         assert wd.address.lo.expr() == lo
         assert wd.address.hi.expr() == hi
         assert wd.amount == bytes_to_fq(cc.pop(0)[::-1])
+
+
+def verify_public_data(public_data: PublicData, MAX_TXS: int, MAX_CALLDATA_BYTES: int, MAX_WITHDRAWALS: int,
+                       ctx: Optional[native.Context] = None) -> PublicInputs:
+    """verify_circuit(public_data2witness(public_data, ...), ...) with the witness built on the device
+    (assign.assign_pi_circuit) and checked where it stands: every row's gates and lookups in one zk_check, failures
+    raised like verify_circuit.  The copy-constraint half of verify_circuit holds by construction here: the tables'
+    cells and the raw bytes it compares are both read from the one raw public-input stream.  Returns the public inputs
+    (the digest computed on the device)."""
+    from . import assign
+
+    ctx = ctx or native.default_context()
+    n, public_inputs = assign.assign_pi_circuit(ctx, public_data, MAX_TXS, MAX_CALLDATA_BYTES, MAX_WITHDRAWALS)
+    ff, _ = ctx.check(native.CIRCUIT_PI, 0, n, 0, native.FLAG_WRAP)
+    raise_first_failure(ff, native.CIRCUIT_PI, "pi row")
+    return public_inputs
 
 
 def verify_circuit(witness: Witness, MAX_TXS: int, MAX_CALLDATA_BYTES: int, MAX_WITHDRAWALS: int,
