@@ -258,10 +258,32 @@ int zk_assign_keccak_table(zk_ctx* ctx, uint64_t n, const uint8_t* data, const u
  *   max_txs CallDataLength fields (big-endian, at their fixed offsets) sum to more than max_calldata_bytes.  A stream
  *   that is otherwise inconsistent (a CallDataGasCost that does not match the calldata, a zero withdrawal amount) is
  *   assigned as it is, and zk_check decides whether it holds.
+ * zk_assign_tx_table = Transaction.table_assignments (evm_circuit/typing.py:209-281) of every tx, the tx table the EVM
+ *   circuit (BeginTx / EndTx, CALLDATALOAD, CALLDATACOPY, ORIGIN, GASPRICE, ...) and the copy circuit's TxCalldata
+ *   rows look up.  txs[n][11][4] = { id, nonce, gas, gas_price, caller_address, callee_address, is_create, value,
+ *   tx_invalid, access_list_gas_cost, tx_sign_hash }, each 4 little-endian limbs; the Word cells (gas_price, caller,
+ *   callee, value) are 256-bit integers, split into (lo, hi) on the device, the others canonical Fr.  Tx k's call data
+ *   is call_data[call_data_offsets[k] .. call_data_offsets[k + 1]).  ZK_TABLE_TX becomes, tx by tx, the 12 fixed rows
+ *   (id, tag 1..12, 0, value lo, hi), with CallDataLength from the offsets and CallDataGasCost (4 per zero byte, 16 per
+ *   other byte) counted on the device, then one (id, CallData = 13, i, byte, 0) row per call-data byte; its row flags
+ *   carry WordOrValue.is_word in bit 0 (tags 3, 4, 5, 7).  Columns are narrow, their widths taken from the record
+ *   maxima.  Indexes cached on the old table are dropped; n_txs = 0 gives an empty table.  Returns -1 before anything
+ *   is stored (the previous table stays in place) when a value cell is >= p, the offsets do not rise from 0, or the
+ *   table would reach 2^31 - 1 rows.
+ * zk_assign_copy_table = Tables._convert_copy_circuit_to_table (evm_circuit/table.py:627-652) over the resident
+ *   ZK_CIRCUIT_COPY, in any storage form (canonical, packed, bound, or zk_assign_copy_circuit's narrow columns):
+ *   ZK_TABLE_COPY becomes one row per circuit row i whose is_first is exactly 1, in circuit order: is_first, id lo,
+ *   hi, tag of row i, id lo, hi, tag of row i + 1, addr of row i, src_addr_end, addr of row i + 1, bytes_left,
+ *   rlc_acc, rw_counter, rwc_inc_left of row i.  Duplicate events give duplicate rows; a lookup counts identical rows
+ *   once, so the table means the reference's set.  The call synchronises `stream` once, after counting the rows: an
+ *   is_first row that is the circuit's last returns -1 with "Not enough rows in copy circuit", an is_first row whose
+ *   next row has q_step != 0 returns -1 with "Invalid copy circuit" (the reference's asserts, the first such row in
+ *   circuit order deciding), and neither touches the previous table.  No resident copy circuit returns -1.
  * zk_download_columns widens the resident matrix of a circuit back to canonical cells
  *   (colmajor_out: uint64[n_cols][zk_resident_rows][4]; flags_out: uint8[rows] or NULL) — inspection and tests.
  *   zk_table_rows / zk_download_table do the same for a resident lookup table
- *   (colmajor_out: uint64[zk_table_cols][zk_table_rows][4]). */
+ *   (colmajor_out: uint64[zk_table_cols][zk_table_rows][4]); zk_download_table_flags copies its row flags
+ *   (flags_out: uint8[zk_table_rows], all zero where the table has none). */
 int zk_assign_bytecode_circuit(zk_ctx* ctx, uint32_t k, uint64_t n_contracts, const uint8_t* code, const uint8_t* is_code_bits,
                                const uint64_t* code_offsets, const uint64_t* hashes, void* stream);
 int zk_assign_state_circuit(zk_ctx* ctx, uint64_t n_rows, const void* packed_ops, uint64_t total_bytes,
@@ -272,10 +294,14 @@ int zk_assign_exp_circuit(zk_ctx* ctx, uint64_t n_events, const uint64_t* events
 int zk_assign_pi_circuit(zk_ctx* ctx, uint64_t max_txs, uint64_t max_calldata_bytes, uint64_t max_withdrawals,
                          const uint8_t* raw_public_inputs, uint64_t n_bytes,
                          uint64_t* pi_keccak_out /* [4]: lo limb0, lo limb1, hi limb0, hi limb1, or NULL */, void* stream);
+int zk_assign_tx_table(zk_ctx* ctx, uint64_t n_txs, const uint64_t* txs /* [n][11][4] */, const uint8_t* call_data,
+                       const uint64_t* call_data_offsets /* [n + 1] */, void* stream);
+int zk_assign_copy_table(zk_ctx* ctx, void* stream);
 int64_t zk_resident_rows(zk_ctx* ctx, int circuit_id);
 int zk_download_columns(zk_ctx* ctx, int circuit_id, uint64_t* colmajor_out, uint8_t* flags_out, void* stream);
 int64_t zk_table_rows(zk_ctx* ctx, int table_id);
 int zk_download_table(zk_ctx* ctx, int table_id, uint64_t* colmajor_out, void* stream);
+int zk_download_table_flags(zk_ctx* ctx, int table_id, uint8_t* flags_out, void* stream);
 
 /* Check rows [row_begin, row_end) of the resident matrix (local indices).  Without
  * ZK_FLAG_WRAP the caller guarantees halo rows exist for the circuit's rotations.

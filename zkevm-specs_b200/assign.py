@@ -2,10 +2,12 @@
 
 The reference builds circuit rows with Python object loops (assign_bytecode_circuit, bytecode_circuit.py:104-167;
 op2row / assign_state_circuit, state_circuit.py:827-889; CopyCircuit.copy, evm_circuit/typing.py:1010-1147;
-ExpCircuit.add_event, evm_circuit/typing.py:880-994; public_data2witness, pi_circuit.py:839-1073).  The functions here
-hand the device the compact data those loops start from — raw code bytes, 15 operation cells, copy events + the copied
-bytes, (base, exponent, identifier) per exponentiation, the raw public-input stream — and leave the expanded witness
-resident for zk_check."""
+ExpCircuit.add_event, evm_circuit/typing.py:880-994; public_data2witness, pi_circuit.py:839-1073;
+Transaction.table_assignments, evm_circuit/typing.py:209-281; Tables._convert_copy_circuit_to_table,
+evm_circuit/table.py:627-652).  The functions here hand the device the compact data those loops start from — raw code
+bytes, 15 operation cells, copy events + the copied bytes, (base, exponent, identifier) per exponentiation, the raw
+public-input stream, 11 cells + the call data per transaction, the resident copy circuit — and leave the expanded
+witness or table resident for zk_check."""
 from __future__ import annotations
 
 from typing import Dict, List, Optional, Sequence
@@ -140,3 +142,53 @@ def assign_pi_circuit(ctx: native.Context, public_data, MAX_TXS: int, MAX_CALLDA
     digest = ctx.assign_pi_circuit(MAX_TXS, MAX_CALLDATA_BYTES, MAX_WITHDRAWALS, raw, stream=stream)
     b = public_data.block
     return len(raw), pc.PublicInputs(Word(digest), Word(b.hash), Word(b.state_root), Word(public_data.state_root_prev))
+
+
+TX_SIGN_HASH = 1234  # the mirror's (and the reference's) mock sign hash, Transaction.table_fixed
+
+
+def tx_records(txs):
+    """evm_circuit.typing.Transaction objects -> the arguments of Context.assign_tx_table: (records uint64[n][11][4], call
+    data uint8, offsets uint64[n + 1]).  A record is id, nonce, gas, gas_price, caller_address, callee_address,
+    is_create, value, tx_invalid, access_list_gas_cost, tx_sign_hash.  Value fields are reduced mod p like FQ(); Word
+    fields (gas_price, caller, callee, value) are checked like Word() (outside [0, 2^256) raises); a creation (callee
+    None) has is_create 1 and callee 0; the access-list gas cost is computed here"""
+    M = (1 << 64) - 1
+    txs = list(txs)
+    rec = np.zeros((len(txs), 11, 4), dtype=np.uint64)
+    fq = lambda x: FQ(packing.cell_int(x)).n  # noqa: E731
+    word = lambda x: Word(int(x)).int_value()  # noqa: E731
+    for k, t in enumerate(txs):
+        callee = t.callee_address
+        cells = (fq(t.id), fq(t.nonce), fq(t.gas), word(t.gas_price), word(t.caller_address),
+                 word(0 if callee is None else callee), int(callee is None), word(t.value), fq(t.invalid_tx),
+                 fq(t.access_list_gas_cost()), TX_SIGN_HASH)
+        for c, v in enumerate(cells):
+            rec[k, c] = [(v >> (64 * i)) & M for i in range(4)]
+    offs = np.zeros(len(txs) + 1, dtype=np.uint64)
+    offs[1:] = np.cumsum([len(t.call_data) for t in txs], dtype=np.uint64)
+    data = np.frombuffer(b"".join(bytes(t.call_data) for t in txs), dtype=np.uint8)
+    return rec, data, offs
+
+
+def assign_tx_table(ctx: native.Context, txs, stream: int = 0) -> None:
+    """Tables(tx_table=set(row for tx in txs for row in tx.table_assignments()), ...) as one device call: the tx table
+    (with its Word type flags) stays resident as ZK_TABLE_TX"""
+    rec, data, offs = tx_records(txs)
+    ctx.assign_tx_table(rec, data, offs, stream=stream)
+
+
+COPY_TABLE_ASSERTS = ("Not enough rows in copy circuit", "Invalid copy circuit")
+
+
+def assign_copy_table(ctx: native.Context, stream: int = 0) -> None:
+    """Tables(copy_circuit=...)'s copy table from the resident copy circuit (uploaded or assigned by
+    assign_copy_circuit) as one device call, left resident as ZK_TABLE_COPY.  The reference's two asserts raise
+    AssertionError with its message, and leave the previous table in place"""
+    try:
+        ctx.assign_copy_table(stream=stream)
+    except native.NativeError as e:
+        for msg in COPY_TABLE_ASSERTS:
+            if f"zk_assign_copy_table: {msg} (rc=-1)" == str(e):
+                raise AssertionError(msg) from None
+        raise

@@ -997,6 +997,89 @@ extern "C" int zk_assign_pi_circuit(zk_ctx* ctx, uint64_t max_txs, uint64_t max_
   return 0;
 }
 
+extern "C" int zk_assign_tx_table(zk_ctx* ctx, uint64_t n_txs, const uint64_t* txs, const uint8_t* call_data,
+                                  const uint64_t* call_data_offsets, void* stream) {
+  CK(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  // everything is validated before the resident table is touched: a rejected call leaves it in place
+  if (!call_data_offsets) return fail_msg(ctx, "tx table: call_data_offsets (n_txs + 1 entries) is required");
+  u64 n_rows;
+  unsigned char width[5];
+  if (const char* why = tx_table_plan(n_txs, (const u64*)txs, (const u64*)call_data_offsets, &n_rows, width)) return fail_msg(ctx, why);
+  const u64 n_cd = call_data_offsets[n_txs];
+  const size_t s_rec = 0, s_cd = up32(n_txs * TX_REC_CELLS * 32), s_off = s_cd + up32(n_cd), s_z = s_off + up32((n_txs + 1) * 8);
+  const size_t s_total = s_z + n_txs * 8 + 32;
+  int rc;
+  if ((rc = ensure_astage(ctx, s_total))) return rc;
+  unsigned char* sg = ctx->astage;
+  if (n_txs) {
+    CK(ctx, cudaMemcpyAsync(sg + s_rec, txs, n_txs * TX_REC_CELLS * 32, cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaMemsetAsync(sg + s_z, 0, n_txs * 8, st));
+  }
+  if (n_cd) CK(ctx, cudaMemcpyAsync(sg + s_cd, call_data, n_cd, cudaMemcpyHostToDevice, st));
+  CK(ctx, cudaMemcpyAsync(sg + s_off, call_data_offsets, (n_txs + 1) * 8, cudaMemcpyHostToDevice, st));
+  Matrix& t = ctx->tab[ZK_TABLE_TX];
+  if ((rc = alloc_narrow(ctx, t, n_rows, 5, width))) return rc;  // a new version: cached indexes are rebuilt
+  if (n_rows > t.flags_cap) {
+    if (t.flags) cudaFree(t.flags);
+    t.flags = nullptr;
+    CK(ctx, cudaMalloc(&t.flags, n_rows));
+    t.flags_cap = n_rows;
+  }
+  t.flags_rows = n_rows;
+  if (n_rows == 0) return 0;
+  TxTableAssign a;
+  a.rec = (const u64*)(sg + s_rec);
+  a.cd = sg + s_cd;
+  a.cd_off = (const u64*)(sg + s_off);
+  a.zeros = (unsigned long long*)(sg + s_z);
+  a.n_txs = n_txs, a.n_rows = n_rows, a.n_cd = n_cd;
+  a.base = (unsigned char*)t.dev;
+  a.flags = t.flags;
+  for (int c = 0; c < 5; c++) a.off[c] = t.off[c], a.width[c] = t.width[c];
+  if (n_cd) k_assign_tx_zeros<<<grid_persistent(ctx, k_assign_tx_zeros, 256, n_cd), 256, 0, st>>>(a);
+  k_assign_tx_rows<<<grid_persistent(ctx, k_assign_tx_rows, 256, n_rows), 256, 0, st>>>(a);
+  return launched(ctx, "k_assign_tx_zeros / k_assign_tx_rows", n_cd ? 2 : 1);
+}
+
+static WitnessDev witness_dev(const Matrix& m);
+extern "C" int zk_assign_copy_table(zk_ctx* ctx, void* stream) {
+  CK(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const Matrix& m = ctx->circ[ZK_CIRCUIT_COPY];
+  if (m.version == 0 || (!m.dev && m.n_rows)) return fail_msg(ctx, "no resident copy circuit");
+  const u64 n = m.n_rows, n_tiles = (n + CT_TILE - 1) / CT_TILE;
+  const size_t s_fail = 0, s_cnt = 32, s_total = s_cnt + n_tiles * 8 + 32;
+  int rc;
+  if ((rc = ensure_astage(ctx, s_total))) return rc;
+  unsigned char* sg = ctx->astage;
+  CopyTableAssign a;
+  a.w = witness_dev(m);
+  a.fail = (unsigned long long*)(sg + s_fail);
+  a.tile_count = (u64*)(sg + s_cnt);
+  CK(ctx, cudaMemsetAsync(a.fail, 0xFF, 8, st));
+  CK(ctx, cudaMemsetAsync(a.fail + 1, 0, 8, st));
+  if (n_tiles) {
+    k_copy_table_count<<<(unsigned)n_tiles, 256, 0, st>>>(a);
+    if ((rc = launched(ctx, "k_copy_table_count"))) return rc;
+  }
+  // the one synchronisation: the asserts are decided, and the table sized, before the resident table is touched
+  unsigned long long h[2];
+  CK(ctx, cudaMemcpyAsync(h, a.fail, 16, cudaMemcpyDeviceToHost, st));
+  CK(ctx, cudaStreamSynchronize(st));
+  if (h[0] != ~0ull) return fail_msg(ctx, h[0] + 1 == n ? "Not enough rows in copy circuit" : "Invalid copy circuit");
+  unsigned char width[14];
+  for (int c = 0; c < 14; c++) width[c] = c == 0 ? 1 : m.width[kCopyTableSrc[c]] ? m.width[kCopyTableSrc[c]] : 32;
+  Matrix& t = ctx->tab[ZK_TABLE_COPY];
+  if ((rc = alloc_narrow(ctx, t, h[1], 14, width))) return rc;  // a new version: cached indexes are rebuilt
+  if (h[1] == 0) return 0;
+  a.base = (unsigned char*)t.dev;
+  for (int c = 0; c < 14; c++) a.off[c] = t.off[c], a.width[c] = t.width[c];
+  k_assign_pi_scan_top<CountScan><<<1, 256, 0, st>>>(CountScan{}, n_tiles, a.tile_count);
+  k_copy_table_write<<<(unsigned)n_tiles, 256, 0, st>>>(a);
+  return launched(ctx, "k_assign_pi_scan_top / k_copy_table_write", 2);
+}
+
 extern "C" int64_t zk_resident_rows(zk_ctx* ctx, int circuit_id) {
   if (circuit_id < 0 || circuit_id >= ZK_N_CIRCUITS) return -1;
   return (int64_t)ctx->circ[circuit_id].n_rows;
@@ -1006,6 +1089,12 @@ extern "C" int64_t zk_table_rows(zk_ctx* ctx, int table_id) {
   return (int64_t)ctx->tab[table_id].n_rows;
 }
 
+// the row flags of a resident matrix (all zero where none are stored), after its cells have been synchronised
+static int download_flags(zk_ctx* ctx, const Matrix& m, uint8_t* flags_out) {
+  if (m.flags_rows == m.n_rows && m.n_rows) CK(ctx, cudaMemcpy(flags_out, m.flags, m.n_rows, cudaMemcpyDeviceToHost));
+  else memset(flags_out, 0, m.n_rows);
+  return 0;
+}
 // a resident matrix widened back to canonical cells on the host (inspection / tests)
 static int download_matrix(zk_ctx* ctx, const Matrix& m, uint64_t* colmajor_out, uint8_t* flags_out, cudaStream_t st) {
   CK(ctx, cudaSetDevice(ctx->device));
@@ -1023,11 +1112,7 @@ static int download_matrix(zk_ctx* ctx, const Matrix& m, uint64_t* colmajor_out,
       memcpy(out + 4 * r, v, 32);
     }
   }
-  if (flags_out) {
-    if (m.flags_rows == m.n_rows && m.n_rows) CK(ctx, cudaMemcpy(flags_out, m.flags, m.n_rows, cudaMemcpyDeviceToHost));
-    else memset(flags_out, 0, m.n_rows);
-  }
-  return 0;
+  return flags_out ? download_flags(ctx, m, flags_out) : 0;
 }
 extern "C" int zk_download_columns(zk_ctx* ctx, int circuit_id, uint64_t* colmajor_out, uint8_t* flags_out, void* stream) {
   if (circuit_id < 0 || circuit_id >= ZK_N_CIRCUITS) return fail_msg(ctx, "bad circuit id");
@@ -1036,6 +1121,12 @@ extern "C" int zk_download_columns(zk_ctx* ctx, int circuit_id, uint64_t* colmaj
 extern "C" int zk_download_table(zk_ctx* ctx, int table_id, uint64_t* colmajor_out, void* stream) {
   if (table_id < 0 || table_id >= ZK_N_TABLES) return fail_msg(ctx, "bad table id");
   return download_matrix(ctx, ctx->tab[table_id], colmajor_out, nullptr, (cudaStream_t)stream);
+}
+extern "C" int zk_download_table_flags(zk_ctx* ctx, int table_id, uint8_t* flags_out, void* stream) {
+  if (table_id < 0 || table_id >= ZK_N_TABLES) return fail_msg(ctx, "bad table id");
+  CK(ctx, cudaSetDevice(ctx->device));
+  CK(ctx, cudaStreamSynchronize((cudaStream_t)stream));
+  return download_flags(ctx, ctx->tab[table_id], flags_out);
 }
 
 // ------------------------------------------------------------------ lookup index cache

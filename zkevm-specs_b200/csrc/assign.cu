@@ -814,6 +814,176 @@ static const char* pi_calldata_offsets(u64 max_txs, u64 max_cd, const unsigned c
   return nullptr;
 }
 
+// ---------------------------------------------------------------- tx table
+// Transaction.table_assignments (evm_circuit/typing.py:209-281) per tx, in tx order: the 12 fixed rows (tags 1..12,
+// call_data_index_or_zero 0), then one (id, CallData, i, byte, 0) row per call-data byte.  Tx k owns rows
+// [12 k + cd_off[k], 12 (k + 1) + cd_off[k + 1]).  A record is 11 cells of 4 little-endian limbs: id, nonce, gas,
+// gas_price, caller_address, callee_address, is_create, value, tx_invalid, access_list_gas_cost, tx_sign_hash; the
+// Word cells (gas_price, caller, callee, value) are 256-bit integers split into (lo, hi) here, the others values.
+// CallDataLength comes from the offsets, CallDataGasCost = 16 len - 12 zeros from the zero-byte counts.
+#define TX_REC_CELLS 11
+#define TX_FIXED_ROWS 12
+#define TX_TAG_CALLDATA 13
+enum { TXR_ID, TXR_NONCE, TXR_GAS, TXR_GAS_PRICE, TXR_CALLER, TXR_CALLEE, TXR_IS_CREATE, TXR_VALUE, TXR_INVALID, TXR_ALGC,
+       TXR_SIGN_HASH };
+struct TxTableAssign {
+  const u64* rec;            // [n_txs][11][4]
+  const unsigned char* cd;   // call data of every tx, back to back
+  const u64* cd_off;         // [n_txs + 1]
+  unsigned long long* zeros;  // [n_txs] zero bytes of each tx's call data (k_assign_tx_zeros)
+  u64 n_txs, n_rows, n_cd;
+  unsigned char* base;  // the table's narrow columns: tx_id, tag, index, value lo, value hi
+  u64 off[5];
+  unsigned char width[5];
+  unsigned char* flags;  // [n_rows] bit 0: the value is a Word
+};
+
+// tag -> the record cell it takes (-1: CallDataLength / CallDataGasCost, from the call data), and whether it is a Word
+ZK_HD int tx_tag_cell(u64 tag) {
+  return tag <= 7 ? (int)tag : tag == 8 || tag == 9 ? -1 : (int)tag - 2;
+}
+ZK_HD bool tx_tag_word(u64 tag) { return tag == 3 || tag == 4 || tag == 5 || tag == 7; }
+ZK_HD void st_width(unsigned char* col, u32 width, u64 row, const Fr& v) {
+  if (width == 32) st_fr(col, row, v);
+  else if (width == 16) st_u128(col, row, v.l[0], v.l[1]);
+  else st_narrow(col, width, row, v.l[0]);
+}
+// the tx whose call data holds byte j (j < n_cd): the largest k < n_txs with cd_off[k] <= j
+ZK_HD u64 tx_of_byte(const TxTableAssign& a, u64 j) {
+  u64 lo = 0, hi = a.n_txs;
+  while (hi - lo > 1) {
+    const u64 mid = (lo + hi) >> 1;
+    if (a.cd_off[mid] <= j) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+ZK_HD void assign_tx_row(const TxTableAssign& a, u64 r) {
+  u64 lo = 0, hi = a.n_txs;  // the largest k with 12 k + cd_off[k] <= r: the tx that holds row r
+  while (hi - lo > 1) {
+    const u64 mid = (lo + hi) >> 1;
+    if (TX_FIXED_ROWS * mid + a.cd_off[mid] <= r) lo = mid;
+    else hi = mid;
+  }
+  const u64 k = lo, local = r - (TX_FIXED_ROWS * k + a.cd_off[k]);
+  const u64* rec = a.rec + 4 * TX_REC_CELLS * k;
+  u64 tag = TX_TAG_CALLDATA, index = 0;
+  Fr vlo = fr_u64(0), vhi = fr_u64(0);
+  bool word = false;
+  if (local < TX_FIXED_ROWS) {
+    tag = local + 1;
+    const u64 len = a.cd_off[k + 1] - a.cd_off[k];
+    const int cell = tx_tag_cell(tag);
+    word = tx_tag_word(tag);
+    if (cell < 0) {
+      vlo = fr_u64(tag == 8 ? len : 16 * len - 12 * (u64)a.zeros[k]);
+    } else {
+      const u64* c = rec + 4 * cell;
+      vlo = Fr{{c[0], c[1], word ? 0 : c[2], word ? 0 : c[3]}};
+      if (word) vhi = Fr{{c[2], c[3], 0, 0}};
+    }
+  } else {
+    index = local - TX_FIXED_ROWS;
+    vlo = fr_u64(a.cd[a.cd_off[k] + index]);
+  }
+  st_width(a.base + a.off[0], a.width[0], r, Fr{{rec[0], rec[1], rec[2], rec[3]}});
+  a.base[a.off[1] + r] = (unsigned char)tag;
+  st_narrow(a.base + a.off[2], a.width[2], r, index);
+  st_width(a.base + a.off[3], a.width[3], r, vlo);
+  st_width(a.base + a.off[4], a.width[4], r, vhi);
+  a.flags[r] = word;
+}
+
+// the width (1, 2, 4, 8, 16 or 32 bytes) that holds a 4-limb value
+static unsigned char tx_cell_width(const u64* v) {
+  if (v[2] | v[3]) return 32;
+  if (v[1]) return 16;
+  return v[0] < (1ull << 8) ? 1 : v[0] < (1ull << 16) ? 2 : v[0] < (1ull << 32) ? 4 : 8;
+}
+static bool tx_fr_canonical(const u64* v) { return fr_lt(Fr{{v[0], v[1], v[2], v[3]}}, Fr{{ZK_P0, ZK_P1, ZK_P2, ZK_P3}}); }
+// host validation and column widths of zk_assign_tx_table (and of the CPU emulation): nullptr with *n_rows and
+// width[5] filled, the reason otherwise.  The widths come from the record maxima and from bounds of the derived
+// cells (CallDataLength <= the longest call data, CallDataGasCost <= 16 times it), as the packer measures ranges.
+static const char* tx_table_plan(u64 n_txs, const u64* rec, const u64* cd_off, u64* n_rows, unsigned char* width) {
+  if (cd_off[0] != 0) return "tx table: call_data_offsets[0] must be 0";
+  u64 max_len = 0;
+  width[0] = 1, width[1] = 1, width[2] = 1, width[3] = 1, width[4] = 1;
+  for (u64 k = 0; k < n_txs; k++) {
+    if (cd_off[k + 1] < cd_off[k]) return "tx table: call_data_offsets must be non-decreasing";
+    max_len = std::max<u64>(max_len, cd_off[k + 1] - cd_off[k]);
+    for (int c = 0; c < TX_REC_CELLS; c++) {
+      const u64* v = rec + 4 * (TX_REC_CELLS * k + c);
+      const bool word = c == TXR_GAS_PRICE || c == TXR_CALLER || c == TXR_CALLEE || c == TXR_VALUE;
+      if (!word && !tx_fr_canonical(v)) return "tx table: a value cell is not canonical (>= p)";
+      if (c == TXR_ID) {
+        width[0] = std::max(width[0], tx_cell_width(v));
+      } else if (word) {
+        const u64 lo[4] = {v[0], v[1], 0, 0}, hi[4] = {v[2], v[3], 0, 0};
+        width[3] = std::max(width[3], tx_cell_width(lo));
+        width[4] = std::max(width[4], tx_cell_width(hi));
+      } else {
+        width[3] = std::max(width[3], tx_cell_width(v));
+      }
+    }
+    if (TX_FIXED_ROWS * (k + 1) + cd_off[k + 1] >= 0x7FFFFFFFull) return "tx table: too many rows (table rows are below 2^31 - 1)";
+  }
+  const u64 bound[4] = {16 * max_len, 0, 0, 0}, idx[4] = {max_len, 0, 0, 0};  // CallDataGasCost, CallDataLength
+  width[3] = std::max(width[3], tx_cell_width(bound));
+  width[2] = std::max(width[2], tx_cell_width(idx));
+  *n_rows = TX_FIXED_ROWS * n_txs + cd_off[n_txs];
+  return nullptr;
+}
+
+// ---------------------------------------------------------------- copy table
+// Tables._convert_copy_circuit_to_table (evm_circuit/table.py:627-652) over the resident copy circuit: every row i whose
+// is_first equals 1 gives one row, in circuit order, of (is_first, id lo, hi, tag, addr, src_addr_end, bytes_left,
+// rlc_acc, rw_counter, rwc_inc_left) of row i and (id lo, hi, tag, addr) of row i + 1 as the destination's.  A stream
+// compaction: k_copy_table_count counts each tile's rows and raises the reference's two asserts as the smallest
+// failing row, the host scans the tile counts (k_assign_pi_scan_top) and k_copy_table_write writes each tile's rows
+// from its offset.
+#define CT_TILE 1024  // circuit rows per block of the two copy-table kernels (256 threads, 4 rows each)
+// the circuit column each table column comes from (table columns 4, 5, 6 and 9 from row i + 1)
+static const unsigned char kCopyTableSrc[14] = {1, 3, 4, 5, 3, 4, 5, 6, 7, 6, 8, 10, 13, 14};
+struct CopyTableAssign {
+  WitnessDev w;  // the resident copy circuit, any storage form
+  u64* tile_count;  // [n_tiles] is_first rows of each tile, then (after the scan) the rows before each tile
+  unsigned long long* fail;  // [0] the smallest row that fails an assert (~0: none), [1] is_first rows in all
+  unsigned char* base;       // the table's narrow columns
+  u64 off[14];
+  unsigned char width[14];
+};
+struct CountScan {
+  typedef u64 T;
+  ZK_HD T id() const { return 0; }
+  static ZK_HD T op(const T& l, const T& r) { return l + r; }
+};
+ZK_HD bool fr_is_one(const Fr& v) { return v.l[0] == 1 && !(v.l[1] | v.l[2] | v.l[3]); }
+ZK_HD bool copy_row_is_first(const CopyTableAssign& a, u64 i) { return i < a.w.n_rows && fr_is_one(wcell(a.w, 1, i)); }
+// an is_first row the reference's conversion asserts on: the last row ("Not enough rows in copy circuit"), or a next
+// row whose q_step is not 0 ("Invalid copy circuit")
+ZK_HD bool copy_row_fails(const CopyTableAssign& a, u64 i) {
+  if (i + 1 == a.w.n_rows) return true;
+  const Fr q = wcell(a.w, 0, i + 1);
+  return (q.l[0] | q.l[1] | q.l[2] | q.l[3]) != 0;
+}
+ZK_HD void copy_table_row(const CopyTableAssign& a, u64 i, u64 pos) {
+  unsigned char* B = a.base;
+  st_width(B + a.off[0], a.width[0], pos, wcell(a.w, 1, i));
+  st_width(B + a.off[1], a.width[1], pos, wcell(a.w, 3, i));
+  st_width(B + a.off[2], a.width[2], pos, wcell(a.w, 4, i));
+  st_width(B + a.off[3], a.width[3], pos, wcell(a.w, 5, i));
+  st_width(B + a.off[4], a.width[4], pos, wcell(a.w, 3, i + 1));
+  st_width(B + a.off[5], a.width[5], pos, wcell(a.w, 4, i + 1));
+  st_width(B + a.off[6], a.width[6], pos, wcell(a.w, 5, i + 1));
+  st_width(B + a.off[7], a.width[7], pos, wcell(a.w, 6, i));
+  st_width(B + a.off[8], a.width[8], pos, wcell(a.w, 7, i));
+  st_width(B + a.off[9], a.width[9], pos, wcell(a.w, 6, i + 1));
+  st_width(B + a.off[10], a.width[10], pos, wcell(a.w, 8, i));
+  st_width(B + a.off[11], a.width[11], pos, wcell(a.w, 10, i));
+  st_width(B + a.off[12], a.width[12], pos, wcell(a.w, 13, i));
+  st_width(B + a.off[13], a.width[13], pos, wcell(a.w, 14, i));
+}
+
 #ifdef __CUDACC__
 __global__ void __launch_bounds__(256) k_seg_local(SegHorner s, Fr* chunk_val) {
   const u64 c = (u64)blockIdx.x * blockDim.x + threadIdx.x;
@@ -920,6 +1090,73 @@ __global__ void __launch_bounds__(256) k_assign_pi_rows(const __grid_constant__ 
 }
 __global__ void __launch_bounds__(32) k_assign_pi_finish(const __grid_constant__ PiAssign a) {
   if (threadIdx.x == 0) assign_pi_finish(a);
+}
+
+// ---- tx table
+// zero call-data bytes per tx, one thread per byte on a persistent grid: the lanes of a warp that hold bytes of the same
+// tx add their zero bytes with one atomic, so a tx of 2^20 bytes costs 2^15 atomics, not one thread walking it
+__global__ void __launch_bounds__(256) k_assign_tx_zeros(const __grid_constant__ TxTableAssign a) {
+  const u32 lane = threadIdx.x & 31;
+  const u64 stride = (u64)gridDim.x * blockDim.x;
+  for (u64 w = (u64)blockIdx.x * blockDim.x + threadIdx.x - lane; w < a.n_cd; w += stride) {  // warp-uniform
+    const u64 j = w + lane;
+    const bool in = j < a.n_cd;
+    const u64 k = in ? tx_of_byte(a, j) : ~0ull;
+    const u32 zero = __ballot_sync(~0u, in && a.cd[j] == 0);
+    const u32 same = __match_any_sync(~0u, k);
+    if (in && lane == (u32)__ffs(same) - 1 && (zero & same)) atomicAdd(a.zeros + k, (unsigned long long)__popc(zero & same));
+  }
+}
+__global__ void __launch_bounds__(256) k_assign_tx_rows(const __grid_constant__ TxTableAssign a) {
+  const u64 stride = (u64)gridDim.x * blockDim.x;
+  for (u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x; r < a.n_rows; r += stride) assign_tx_row(a, r);
+}
+
+// ---- copy table
+// per tile of CT_TILE circuit rows: its is_first rows, the smallest row failing an assert, the total
+__global__ void __launch_bounds__(256) k_copy_table_count(const __grid_constant__ CopyTableAssign a) {
+  __shared__ u32 cnt;
+  if (threadIdx.x == 0) cnt = 0;
+  __syncthreads();
+  u32 mine = 0;
+#pragma unroll
+  for (int q = 0; q < CT_TILE / 256; q++) {
+    const u64 i = (u64)blockIdx.x * CT_TILE + q * 256 + threadIdx.x;
+    if (copy_row_is_first(a, i)) {
+      mine++;
+      if (copy_row_fails(a, i)) atomicMin(a.fail, (unsigned long long)i);
+    }
+  }
+  for (int o = 16; o; o >>= 1) mine += __shfl_down_sync(~0u, mine, o);
+  if ((threadIdx.x & 31) == 0 && mine) atomicAdd(&cnt, mine);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    a.tile_count[blockIdx.x] = cnt;
+    if (cnt) atomicAdd(a.fail + 1, (unsigned long long)cnt);
+  }
+}
+// after the exclusive scan of the tile counts: each tile's is_first rows, in circuit order, from its offset
+__global__ void __launch_bounds__(256) k_copy_table_write(const __grid_constant__ CopyTableAssign a) {
+  __shared__ u32 warp_n[8];
+  const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  u64 pos = a.tile_count[blockIdx.x];
+  for (int q = 0; q < CT_TILE / 256; q++) {
+    const u64 i = (u64)blockIdx.x * CT_TILE + q * 256 + threadIdx.x;
+    const bool f = copy_row_is_first(a, i);
+    const u32 b = __ballot_sync(~0u, f);
+    if (lane == 0) warp_n[warp] = __popc(b);
+    __syncthreads();
+    u32 before = 0, total = 0;
+#pragma unroll
+    for (u32 v = 0; v < 8; v++) {
+      const u32 n = warp_n[v];
+      before += v < warp ? n : 0;
+      total += n;
+    }
+    if (f) copy_table_row(a, i, pos + before + __popc(b & ((1u << lane) - 1)));
+    pos += total;
+    __syncthreads();
+  }
 }
 #endif
 

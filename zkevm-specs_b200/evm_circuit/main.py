@@ -132,10 +132,19 @@ def verify_steps(tables: Tables, steps: List[StepState], begin_with_first_step: 
     """Reference signature and error convention (main.py:14-44): mutates `steps` when
     end_with_last_step; an AssertionError-class failure is re-raised when success=True and
     required when success=False; every other failure class propagates."""
-    if end_with_last_step:
-        steps.append(DUMMY_STEP_STATE)
     ctx = ctx or native.default_context()
     upload_tables(ctx, tables)
+    verify_steps_resident(steps, ctx, begin_with_first_step, end_with_last_step, success)
+
+
+def verify_steps_resident(steps: List[StepState], ctx: native.Context, begin_with_first_step: bool = False,
+                          end_with_last_step: bool = False, success: bool = True) -> None:
+    """verify_steps against the tables already resident in `ctx` (uploaded, or built on the device: assign.assign_tx_table,
+    assign_copy_table, assign_exp_circuit, ...): only the steps and their step-aux table are uploaded (and the fixed
+    table, once per context).  Same error convention, and `steps` is mutated the same way"""
+    if end_with_last_step:
+        steps.append(DUMMY_STEP_STATE)
+    upload_fixed_table(ctx)
     ctx.upload_table(native.TABLE_STEP_AUX, packing.matrix_from_ints(step_aux_rows(steps), 3))
     ff, _ = check_steps(ctx, pack_steps(steps), begin_with_first_step, end_with_last_step)
     exception = None

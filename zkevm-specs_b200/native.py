@@ -76,7 +76,7 @@ EXPORTS = [
     "zk_upload_bytecode_table_from_code", "zk_nccl_unique_id", "zk_nccl_comm_init", "zk_nccl_comm_destroy",
     "zk_keccak256_batch", "zk_assign_keccak_table", "zk_assign_bytecode_circuit", "zk_assign_state_circuit",
     "zk_assign_copy_circuit", "zk_download_columns", "zk_resident_rows", "zk_assign_exp_circuit", "zk_table_rows",
-    "zk_download_table", "zk_assign_pi_circuit",
+    "zk_download_table", "zk_assign_pi_circuit", "zk_assign_tx_table", "zk_assign_copy_table", "zk_download_table_flags",
 ]
 
 
@@ -123,6 +123,9 @@ def lib() -> ctypes.CDLL:
         L.zk_table_rows.restype = ctypes.c_int64
         L.zk_download_table.argtypes = [vp, i32, vp, vp]
         L.zk_assign_pi_circuit.argtypes = [vp, u64, u64, u64, vp, u64, vp, vp]
+        L.zk_assign_tx_table.argtypes = [vp, u64, vp, vp, vp, vp]
+        L.zk_assign_copy_table.argtypes = [vp, vp]
+        L.zk_download_table_flags.argtypes = [vp, i32, vp, vp]
         L.zk_circuit_cols.argtypes = [i32]
         L.zk_table_cols.argtypes = [i32]
         L.zk_n_constraints.argtypes = [i32]
@@ -318,6 +321,23 @@ class Context:
             return None
         return sum(int(x) << (64 * i) for i, x in enumerate(out))
 
+    def assign_tx_table(self, records: np.ndarray, call_data, call_data_offsets: np.ndarray, stream: int = 0) -> None:
+        """Transaction.table_assignments (evm_circuit/typing.py:209-281) of every tx on the device: `records` uint64[n][11][4]
+        (assign.tx_records), `call_data` the txs' call data back to back (bytes or uint8), `call_data_offsets` uint64[n + 1].
+        The table REPLACES the resident TABLE_TX, with its Word type flags"""
+        rec = np.ascontiguousarray(records, dtype=np.uint64).reshape(-1, 11, 4)
+        cd = np.frombuffer(bytes(call_data), dtype=np.uint8) if not isinstance(call_data, np.ndarray) else np.ascontiguousarray(call_data, dtype=np.uint8)
+        offs = np.ascontiguousarray(call_data_offsets, dtype=np.uint64)
+        assert offs.shape == (rec.shape[0] + 1,) and (rec.shape[0] == 0 or int(offs[-1]) <= len(cd))
+        self._ck(self._L.zk_assign_tx_table(self._h, rec.shape[0], _host_ptr(rec), _host_ptr(cd) if len(cd) else None,
+                                            _host_ptr(offs), ctypes.c_void_p(stream)), "zk_assign_tx_table")
+
+    def assign_copy_table(self, stream: int = 0) -> None:
+        """Tables._convert_copy_circuit_to_table (evm_circuit/table.py:627-652) over the resident CIRCUIT_COPY, on the
+        device: the table REPLACES the resident TABLE_COPY.  Waits for the stream once; the reference's two asserts
+        raise NativeError with its message and leave the previous table in place"""
+        self._ck(self._L.zk_assign_copy_table(self._h, ctypes.c_void_p(stream)), "zk_assign_copy_table")
+
     def download_columns(self, circuit_id: int, stream: int = 0):
         """the resident matrix of a circuit as canonical cells + its row flags: (uint64[n_cols][n_rows][4], uint8[n_rows])"""
         n_cols, n_rows = self._L.zk_circuit_cols(circuit_id), self.resident_rows(circuit_id)
@@ -335,6 +355,13 @@ class Context:
         out = np.zeros((self._L.zk_table_cols(table_id), self.table_rows(table_id), 4), dtype=np.uint64)
         self._ck(self._L.zk_download_table(self._h, table_id, _host_ptr(out), ctypes.c_void_p(stream)), "zk_download_table")
         return out
+
+    def download_table_flags(self, table_id: int, stream: int = 0) -> np.ndarray:
+        """the row flags of a resident lookup table: uint8[n_rows] (zeros where it has none)"""
+        out = np.zeros(max(self.table_rows(table_id), 1), dtype=np.uint8)
+        self._ck(self._L.zk_download_table_flags(self._h, table_id, _host_ptr(out), ctypes.c_void_p(stream)),
+                 "zk_download_table_flags")
+        return out[:self.table_rows(table_id)]
 
     def table_rows(self, table_id: int) -> int:
         return int(self._L.zk_table_rows(self._h, table_id))
