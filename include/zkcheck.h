@@ -227,6 +227,21 @@ int zk_assign_keccak_table(zk_ctx* ctx, uint64_t n, const uint8_t* data, const u
  *   (zk_upload_columns_packed); the ten 16-bit address limbs and the 32 storage-key bytes of the 57-cell row are
  *   derived on the device.  An address beyond 160 bits is an error (the reference raises OverflowError).
  *   row_flags as zk_upload_row_flags (may be NULL).
+ * zk_assign_state_circuit_mpt = assign_state_circuit with its mock MPT updates (state_circuit.py:861-933) from the
+ *   operations alone: `packed_ops` holds the 13 cells an operation brings (the 15 of zk_assign_state_circuit without
+ *   root lo, hi), row_flags as there (bit 0: the value is a Word, bit 1: the initial value is; NULL: all field values).
+ *   ZK_CIRCUIT_STATE becomes the n 57-cell rows zk_assign_state_circuit gives with the reference's roots: row k's root
+ *   is root_prev of the update of the first Account (tag 6) or Storage (tag 4) op after k, or the final root 3 + 5U
+ *   (root lo a narrow column, root hi 0).  ZK_TABLE_MPT becomes the U updates in first-touch order: one per distinct
+ *   key (address, field_tag, storage_key lo, hi) of those ops, from its first op: (address, proof type = 6 for Storage
+ *   or the Account field tag, key lo, hi, root 3 + 5(u + 1), 0, root_prev 3 + 5u, 0, value lo, hi, value_prev lo, hi)
+ *   with the value and initial value as Word(int_value()): a field value split at 2^128, a Word lo + hi 2^128
+ *   re-split.  *n_updates_out (may be NULL) = U.  Computed on the device (a hash table of first touches per key and
+ *   two count scans); the call synchronises the stream once.  Returns -1 and keeps the previous matrix and table for
+ *   the row bound, an address beyond 160 bits (checked on the host first; the mirror would name an MPT error first on
+ *   an input that has both), and, decided by the first failing op in operation order, a first-touch Account op whose
+ *   field tag is not 1..4 (the mirror's KeyError) or a first-touch op whose Word value or initial value is >= 2^256
+ *   (Word() asserts).
  * zk_assign_copy_circuit = CopyCircuit.copy per event (evm_circuit/typing.py:1010-1147): events[n][16] =
  *   { src_tag | src id is a Word << 8, dst_tag | dst id is a Word << 8, src_addr, src_addr_end, dst_addr, copy_length,
  *   log_id, rw_counter before the event, src_id lo (2 limbs), hi (2 limbs), dst_id lo (2 limbs), hi (2 limbs) };
@@ -288,6 +303,9 @@ int zk_assign_bytecode_circuit(zk_ctx* ctx, uint32_t k, uint64_t n_contracts, co
                                const uint64_t* code_offsets, const uint64_t* hashes, void* stream);
 int zk_assign_state_circuit(zk_ctx* ctx, uint64_t n_rows, const void* packed_ops, uint64_t total_bytes,
                             const uint64_t* col_offsets, const uint8_t* col_widths, const uint8_t* row_flags, void* stream);
+int zk_assign_state_circuit_mpt(zk_ctx* ctx, uint64_t n_rows, const void* packed_ops, uint64_t total_bytes,
+                                const uint64_t* col_offsets /* [13] */, const uint8_t* col_widths /* [13] */,
+                                const uint8_t* row_flags, uint64_t* n_updates_out, void* stream);
 int zk_assign_copy_circuit(zk_ctx* ctx, uint64_t n_events, const uint64_t* events, const uint8_t* data,
                            const uint8_t* is_code_bits, void* stream);
 int zk_assign_exp_circuit(zk_ctx* ctx, uint64_t n_events, const uint64_t* events, uint64_t n_rows_min, void* stream);

@@ -1,13 +1,14 @@
 """Witness assignment on the device — host side of include/zkcheck.h "witness assignment" (csrc/assign.cu).
 
 The reference builds circuit rows with Python object loops (assign_bytecode_circuit, bytecode_circuit.py:104-167;
-op2row / assign_state_circuit, state_circuit.py:827-889; CopyCircuit.copy, evm_circuit/typing.py:1010-1147;
-ExpCircuit.add_event, evm_circuit/typing.py:880-994; public_data2witness, pi_circuit.py:839-1073;
-Transaction.table_assignments, evm_circuit/typing.py:209-281; Tables._convert_copy_circuit_to_table,
-evm_circuit/table.py:627-652).  The functions here hand the device the compact data those loops start from — raw code
-bytes, 15 operation cells, copy events + the copied bytes, (base, exponent, identifier) per exponentiation, the raw
-public-input stream, 11 cells + the call data per transaction, the resident copy circuit — and leave the expanded
-witness or table resident for zk_check."""
+op2row / assign_state_circuit and its mock MPT updates, state_circuit.py:827-933; CopyCircuit.copy,
+evm_circuit/typing.py:1010-1147; ExpCircuit.add_event, evm_circuit/typing.py:880-994; public_data2witness,
+pi_circuit.py:839-1073; Transaction.table_assignments, evm_circuit/typing.py:209-281;
+Tables._convert_copy_circuit_to_table, evm_circuit/table.py:627-652).  The functions here hand the device the compact
+data those loops start from — raw code bytes, 15 operation cells (or 13, the roots and the MPT table then built on the
+device), copy events + the copied bytes, (base, exponent, identifier) per exponentiation, the raw public-input stream,
+11 cells + the call data per transaction, the resident copy circuit — and leave the expanded witness or table resident
+for zk_check."""
 from __future__ import annotations
 
 from typing import Dict, List, Optional, Sequence
@@ -15,7 +16,7 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 
 from . import native, packing
-from .evm_circuit.spec import CopyDataTypeTag
+from .evm_circuit.spec import RW, CopyDataTypeTag
 from .util.arithmetic import FQ, Word
 from .util.hash import keccak256
 
@@ -72,6 +73,47 @@ def assign_state_circuit(ctx: native.Context, ops, flags=None, stream: int = 0) 
         cols, flags = sc.pack_rows(rows)  # host op2row only to read the 15 operation cells and the roots
         m = state_ops_from_rows(cols)
     ctx.assign_state_circuit(packing.pack_matrix(m), flags=flags, stream=stream)
+
+
+STATE_OP13_COLS = list(range(8)) + [50, 51, 52, 53, 56]  # the 13 cells of a state row an operation brings: no root
+
+
+def state_op13_from_rows(rows57: np.ndarray) -> np.ndarray:
+    """the operation cells of packed state rows without the root: uint64[57][n][4] -> uint64[13][n][4]"""
+    return np.ascontiguousarray(rows57[STATE_OP13_COLS])
+
+
+def state_op_cells(ops):
+    """state_circuit.Operation objects -> (uint64[13][n][4], flags uint8[n]): the 13 cells and the WordOrValue type bits
+    the operations bring, without op2row or the MPT walk"""
+    c = packing.cell_int
+    rows = [[int(op.rw_counter), 0 if op.rw == RW.Read else 1, int(op.tag), int(op.id), int(op.address), int(op.field_tag),
+             int(op.storage_key) & ((1 << 128) - 1), int(op.storage_key) >> 128, c(op.value.lo), c(op.value.hi),
+             c(op.initial_value.lo), c(op.initial_value.hi), c(op.lexicographic_ordering_selector)] for op in ops]
+    flags = np.array([packing.word_flag(op.value) | (packing.word_flag(op.initial_value) << 1) for op in ops], dtype=np.uint8)
+    return packing.matrix_from_ints(rows, 13), flags
+
+
+# the two data rejections of zk_assign_state_circuit_mpt and the exception the mirror's _mock_mpt_updates raises there
+STATE_MPT_ERRORS = (("the Account field tag is not Nonce, Balance, CodeHash or NonExisting", KeyError),
+                    ("a Word value or initial value is >= 2^256", AssertionError))
+
+
+def assign_state_circuit_mpt(ctx: native.Context, ops, flags=None, stream: int = 0) -> int:
+    """state_circuit.assign_state_circuit(ops) and mpt_table_from_ops(ops) as one device call: the rows stay resident as
+    ZK_CIRCUIT_STATE, the MPT updates (first-touch order) as ZK_TABLE_MPT; returns their number.  `ops`: a list of
+    state_circuit.Operation, or the 13 operation cells uint64[13][n][4] (or a PackedMatrix of them) with `flags`.  An
+    Account field tag without a proof type raises KeyError, a Word value >= 2^256 AssertionError, as the mirror does;
+    the previous matrix and table stay in place"""
+    if not isinstance(ops, (np.ndarray, packing.PackedMatrix)):
+        ops, flags = state_op_cells(list(ops))
+    try:
+        return ctx.assign_state_circuit_mpt(ops, flags=flags, stream=stream)
+    except native.NativeError as e:
+        for msg, exc in STATE_MPT_ERRORS:
+            if msg in str(e):
+                raise exc(str(e)) from None
+        raise
 
 
 def copy_event(src_id, src_tag, dst_id, dst_tag, src_addr: int, src_addr_end: int, dst_addr: int, copy_length: int,

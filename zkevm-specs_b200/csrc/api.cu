@@ -760,27 +760,16 @@ extern "C" int zk_assign_bytecode_circuit(zk_ctx* ctx, uint32_t k, uint64_t n_co
   return launched(ctx, "k_assign_bytecode_rows / k_assign_bytecode_rlc", n_chunks ? 2 : 1);
 }
 
-extern "C" int zk_assign_state_circuit(zk_ctx* ctx, uint64_t n_rows, const void* packed_ops, uint64_t total_bytes,
-                                       const uint64_t* col_offsets, const uint8_t* col_widths, const uint8_t* row_flags,
-                                       void* stream) {
-  CK(ctx, cudaSetDevice(ctx->device));
-  cudaStream_t st = (cudaStream_t)stream;
-  if (n_rows >= 0xFFFFFFFFull) return fail_msg(ctx, "too many rows (row ids are uint32)");
-  if (!col_offsets || !col_widths) return fail_msg(ctx, "zk_assign_state_circuit needs offsets and widths of the 15 operation columns");
-  for (int c = 0; c < 15; c++) {
-    const unsigned w = col_widths[c];
-    if (!(w == 0 || w == 1 || w == 2 || w == 4 || w == 8 || w == 16 || w == 32)) return fail_msg(ctx, "packed column width must be 0, 1, 2, 4, 8, 16 or 32");
-    if (col_offsets[c] % 32 || col_offsets[c] + (w ? (size_t)w * n_rows : 32) > total_bytes)
-      return fail_msg(ctx, "packed column offset misaligned or outside the buffer");
-  }
-  if (col_widths[4] == 32) {  // op.address.to_bytes(20, "little") raises OverflowError beyond 160 bits (state_circuit.py:832)
-    const u64* a = (const u64*)((const unsigned char*)packed_ops + col_offsets[4]);
-    for (u64 r = 0; r < n_rows; r++)
-      if ((a[4 * r + 2] >> 32) || a[4 * r + 3]) return fail_msg(ctx, "operation address does not fit 20 bytes (op2row raises OverflowError)");
-  }
-  // resident buffer: [uploaded operation columns | 10 limb columns (u16) | 32 key-byte columns (u8)]
+// The resident state matrix from validated operation columns: `copy_bytes` of `ops` (host memory, or device memory
+// when ops_on_device) become the front `front` bytes of the buffer, where off[15] / width[15] locate the 15 operation
+// cells of a row; op2row fills the address limbs and key bytes.  The front may hold more than what is copied (the
+// root columns zk_assign_state_circuit_mpt writes afterwards).
+static int state_rows_from_ops(zk_ctx* ctx, uint64_t n_rows, const void* ops, size_t copy_bytes, bool ops_on_device,
+                               size_t front, const u64* col_offsets, const uint8_t* col_widths, const uint8_t* row_flags,
+                               cudaStream_t st) {
+  // resident buffer: [operation columns | 10 limb columns (u16) | 32 key-byte columns (u8)]
   Matrix& m = ctx->circ[ZK_CIRCUIT_STATE];
-  const size_t front = up32(total_bytes), limb_stride = up32(2 * n_rows), byte_stride = up32(n_rows);
+  const size_t limb_stride = up32(2 * n_rows), byte_stride = up32(n_rows);
   const size_t bytes = front + 10 * limb_stride + 32 * byte_stride;
   if (m.borrowed) {
     m.dev = nullptr;
@@ -793,7 +782,8 @@ extern "C" int zk_assign_state_circuit(zk_ctx* ctx, uint64_t n_rows, const void*
     CK(ctx, cudaMalloc(&m.dev, bytes ? bytes : 32));
     m.cap_bytes = bytes;
   }
-  if (total_bytes) CK(ctx, cudaMemcpyAsync(m.dev, packed_ops, total_bytes, cudaMemcpyHostToDevice, st));
+  if (copy_bytes)
+    CK(ctx, cudaMemcpyAsync(m.dev, ops, copy_bytes, ops_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
   m.version++;
   m.n_rows = n_rows;
   m.n_cols = 57;
@@ -814,6 +804,14 @@ extern "C" int zk_assign_state_circuit(zk_ctx* ctx, uint64_t n_rows, const void*
   a.n_rows = n_rows, a.limb_stride = limb_stride, a.byte_stride = byte_stride;
   k_assign_state_derive<<<(unsigned)std::min<u64>((n_rows + 255) / 256, (u64)ctx->sm_count * 16), 256, 0, st>>>(a);
   return launched(ctx, "k_assign_state_derive");
+}
+extern "C" int zk_assign_state_circuit(zk_ctx* ctx, uint64_t n_rows, const void* packed_ops, uint64_t total_bytes,
+                                       const uint64_t* col_offsets, const uint8_t* col_widths, const uint8_t* row_flags,
+                                       void* stream) {
+  CK(ctx, cudaSetDevice(ctx->device));
+  if (const char* why = state_ops_error(n_rows, 15, packed_ops, total_bytes, col_offsets, col_widths)) return fail_msg(ctx, why);
+  return state_rows_from_ops(ctx, n_rows, packed_ops, total_bytes, false, up32(total_bytes), (const u64*)col_offsets,
+                             col_widths, row_flags, (cudaStream_t)stream);
 }
 
 extern "C" int zk_assign_copy_circuit(zk_ctx* ctx, uint64_t n_events, const uint64_t* events, const uint8_t* data,
@@ -1078,6 +1076,96 @@ extern "C" int zk_assign_copy_table(zk_ctx* ctx, void* stream) {
   k_assign_pi_scan_top<CountScan><<<1, 256, 0, st>>>(CountScan{}, n_tiles, a.tile_count);
   k_copy_table_write<<<(unsigned)n_tiles, 256, 0, st>>>(a);
   return launched(ctx, "k_assign_pi_scan_top / k_copy_table_write", 2);
+}
+
+extern "C" int zk_assign_state_circuit_mpt(zk_ctx* ctx, uint64_t n_rows, const void* packed_ops, uint64_t total_bytes,
+                                           const uint64_t* col_offsets, const uint8_t* col_widths, const uint8_t* row_flags,
+                                           uint64_t* n_updates_out, void* stream) {
+  CK(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  if (const char* why = state_ops_error(n_rows, 13, packed_ops, total_bytes, col_offsets, col_widths)) return fail_msg(ctx, why);
+  const u64 n = n_rows, cap = state_mpt_slots(n), n_chunks = (n + ZK_SEG_CHUNK - 1) / ZK_SEG_CHUNK;
+  const u64 n_blocks = (n_chunks + PI_SCAN_BLOCK_CHUNKS - 1) / PI_SCAN_BLOCK_CHUNKS;
+  // staging: [operation columns | row flags | slots | key minima | ranks | slot of each op | op flags | stat | two count
+  // scans (chunk carries, block carries) | update ops | MPT ops]
+  const size_t s_fl = up32(total_bytes), s_slots = s_fl + up32(n), s_min = s_slots + cap * 8, s_rank = s_min + cap * 4;
+  const size_t s_slot_of = s_rank + cap * 4, s_opfl = s_slot_of + up32(n * 4), s_stat = s_opfl + up32(n);
+  const size_t s_xu = s_stat + 32, s_tu = s_xu + up32(n_chunks * 8), s_xm = s_tu + up32(n_blocks * 8 + 8);
+  const size_t s_tm = s_xm + up32(n_chunks * 8), s_upd = s_tm + up32(n_blocks * 8 + 8), s_mpt = s_upd + up32(n * 4);
+  const size_t s_total = s_mpt + up32(n * 4) + 32;
+  int rc;
+  if ((rc = ensure_astage(ctx, s_total))) return rc;
+  unsigned char* sg = ctx->astage;
+  StateMpt a;
+  a.base = sg;
+  for (int c = 0; c < 13; c++) a.off[c] = col_offsets[c], a.w[c] = col_widths[c];
+  a.flags = row_flags ? sg + s_fl : nullptr;
+  a.n = n;
+  a.slots = (u64*)(sg + s_slots);
+  a.key_min = (u32*)(sg + s_min);
+  a.rank_at = (u32*)(sg + s_rank);
+  a.mask = cap - 1;
+  a.slot_of = (u32*)(sg + s_slot_of);
+  a.fl = sg + s_opfl;
+  a.stat = (unsigned long long*)(sg + s_stat);
+  a.x_upd = (const u64*)(sg + s_xu), a.top_upd = (const u64*)(sg + s_tu);
+  a.x_mpt = (const u64*)(sg + s_xm), a.top_mpt = (const u64*)(sg + s_tm);
+  a.upd_op = (u32*)(sg + s_upd);
+  a.mpt_op = (u32*)(sg + s_mpt);
+  if (total_bytes) CK(ctx, cudaMemcpyAsync(sg, packed_ops, total_bytes, cudaMemcpyHostToDevice, st));
+  if (row_flags && n) CK(ctx, cudaMemcpyAsync(sg + s_fl, row_flags, n, cudaMemcpyHostToDevice, st));
+  CK(ctx, cudaMemsetAsync(sg + s_slots, 0xFF, cap * 12, st));  // slots and key minima: empty
+  CK(ctx, cudaMemsetAsync(a.stat, 0xFF, 8, st));
+  CK(ctx, cudaMemsetAsync(a.stat + 1, 0, 16, st));
+  if (n) {
+    k_state_mpt_insert<<<grid_persistent(ctx, k_state_mpt_insert, 256, n), 256, 0, st>>>(a);
+    k_state_mpt_first<<<grid_persistent(ctx, k_state_mpt_first, 256, n), 256, 0, st>>>(a);
+    if ((rc = launched(ctx, "k_state_mpt_insert / k_state_mpt_first", 2))) return rc;
+    if ((rc = pi_scan(ctx, CountScan{a.fl, n, 2}, (u64*)a.x_upd, (u64*)a.top_upd, st))) return rc;
+    if ((rc = pi_scan(ctx, CountScan{a.fl, n, 1}, (u64*)a.x_mpt, (u64*)a.top_mpt, st))) return rc;
+  }
+  // the one synchronisation: the rejections are decided, and the table sized, before anything resident is touched
+  unsigned long long h[3];
+  CK(ctx, cudaMemcpyAsync(h, a.stat, 24, cudaMemcpyDeviceToHost, st));
+  CK(ctx, cudaStreamSynchronize(st));
+  if (h[0] != ~0ull) {
+    const std::string op = "state circuit: operation " + std::to_string(h[0] >> 2) + ": ";
+    if ((h[0] & 3) == SM_FAIL_FIELD_TAG)
+      return fail_msg(ctx, op + "the Account field tag is not Nonce, Balance, CodeHash or NonExisting (no MPT proof type)");
+    return fail_msg(ctx, op + "a Word value or initial value is >= 2^256");
+  }
+  a.n_upd = h[1], a.n_mpt = h[2];
+  // the 13 columns, then root lo (8 bytes per row) and root hi (a constant 0), in front of the limbs and key bytes
+  const size_t s_root = up32(total_bytes), s_root_hi = s_root + up32(n * 8), front = s_root_hi + 32;
+  u64 off15[15];
+  uint8_t w15[15];
+  for (int c = 0; c < 12; c++) off15[c] = col_offsets[c], w15[c] = col_widths[c];
+  off15[12] = s_root, w15[12] = 8;
+  off15[13] = s_root_hi, w15[13] = 0;
+  off15[14] = col_offsets[12], w15[14] = col_widths[12];
+  if ((rc = state_rows_from_ops(ctx, n, sg, total_bytes, true, front, off15, w15, row_flags, st))) return rc;
+  Matrix& m = ctx->circ[ZK_CIRCUIT_STATE];
+  CK(ctx, cudaMemsetAsync((unsigned char*)m.dev + s_root_hi, 0, 32, st));
+  unsigned char tw[12] = {32, 1, 32, 32, 8, 1, 8, 1, 16, 16, 16, 16};
+  for (int c = 0; c < 3; c++) {  // address, key lo, key hi keep the width they came in (0, a constant, is stored per row)
+    const unsigned w = col_widths[c == 0 ? SO_ADDR : SO_KLO + c - 1];
+    tw[c == 0 ? 0 : c + 1] = (unsigned char)(w ? w : 32);
+  }
+  Matrix& t = ctx->tab[ZK_TABLE_MPT];
+  if ((rc = alloc_narrow(ctx, t, a.n_upd, 12, tw))) return rc;  // a new version: cached indexes are rebuilt
+  if (n_updates_out) *n_updates_out = a.n_upd;
+  if (n == 0) return 0;
+  a.root = (unsigned char*)m.dev + s_root;
+  a.tbase = (unsigned char*)t.dev;
+  for (int c = 0; c < 12; c++) a.toff[c] = t.off[c], a.twidth[c] = t.width[c];
+  k_state_mpt_compact<<<grid_persistent(ctx, k_state_mpt_compact, 256, n), 256, 0, st>>>(a);
+  k_state_mpt_rows<<<grid_persistent(ctx, k_state_mpt_rows, 256, n), 256, 0, st>>>(a);
+  int n_launch = 2;
+  if (a.n_upd) {
+    k_state_mpt_table<<<grid_persistent(ctx, k_state_mpt_table, 256, a.n_upd), 256, 0, st>>>(a);
+    n_launch = 3;
+  }
+  return launched(ctx, "k_state_mpt_compact / k_state_mpt_rows / k_state_mpt_table", n_launch);
 }
 
 extern "C" int64_t zk_resident_rows(zk_ctx* ctx, int circuit_id) {

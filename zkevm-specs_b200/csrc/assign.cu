@@ -3,6 +3,8 @@
 //
 //   assign_bytecode_circuit  src/zkevm_specs/bytecode_circuit.py:104-167   raw code bytes -> 12-cell rows
 //   op2row / assign_state_circuit  src/zkevm_specs/state_circuit.py:827-889  15 operation cells -> 57-cell rows
+//                            + _mock_mpt_updates (state_circuit.py:903-933): 13 operation cells -> the same rows with
+//                            their roots, and the MPT table
 //   CopyCircuit.copy         src/zkevm_specs/evm_circuit/typing.py:1010-1147 copy events + bytes -> 20-cell rows
 //   ExpCircuit.add_event     src/zkevm_specs/evm_circuit/typing.py:880-994  (base, exponent, id) -> 21-cell rows
 //                            + the exp table (Tables._convert_exp_circuit_to_table, table.py:654-671)
@@ -952,9 +954,19 @@ struct CopyTableAssign {
   u64 off[14];
   unsigned char width[14];
 };
+// a count: as the PI scan's monoid over `flags`, fold(lo, hi) counts the items in [lo, hi) with a bit of `mask` set
+// (k_assign_pi_scan); the copy table scans its tile counts with k_assign_pi_scan_top only, which never folds
 struct CountScan {
   typedef u64 T;
+  const unsigned char* flags;
+  u64 n;
+  unsigned mask;
   ZK_HD T id() const { return 0; }
+  ZK_HD T fold(u64 lo, u64 hi) const {
+    u64 c = 0;
+    for (u64 j = lo; j < hi; j++) c += (flags[j] & mask) != 0;
+    return c;
+  }
   static ZK_HD T op(const T& l, const T& r) { return l + r; }
 };
 ZK_HD bool fr_is_one(const Fr& v) { return v.l[0] == 1 && !(v.l[1] | v.l[2] | v.l[3]); }
@@ -982,6 +994,205 @@ ZK_HD void copy_table_row(const CopyTableAssign& a, u64 i, u64 pos) {
   st_width(B + a.off[11], a.width[11], pos, wcell(a.w, 10, i));
   st_width(B + a.off[12], a.width[12], pos, wcell(a.w, 13, i));
   st_width(B + a.off[13], a.width[13], pos, wcell(a.w, 14, i));
+}
+
+// ---------------------------------------------------------------- state circuit roots + MPT table
+// _mock_mpt_updates (state_circuit.py:903-933) walks the operations once, keeping the first touch of each MPT key
+// (address, field_tag, storage_key lo, hi) of an Account or Storage op; update u (first-touch order) moves the root
+// from 3 + 5u to 3 + 5(u + 1).  assign_state_circuit (:861-889) gives row k root_prev of the update of the first MPT op
+// after k, or the final root 3 + 5U.  Here: an open-addressing hash table over the MPT ops keeps the smallest op
+// index per key (an op is a first touch when it is its key's minimum), count scans over the first-touch and MPT-op
+// flags rank the updates and list the MPT ops in order, and every row and table row is then a closed form.
+#define SM_EMPTY 0xFFFFFFFFFFFFFFFFull  // a slot is (hash32 << 32) | op index of the op that claimed it
+#define SM_TAG_STORAGE 4
+#define SM_TAG_ACCOUNT 6
+#define SM_PROOF_STORAGE_MOD 6
+#define SM_FAIL_FIELD_TAG 1  // a first-touch Account op's field tag is not 1..4 (the mirror's KeyError)
+#define SM_FAIL_WORD 2       // a first-touch op's Word value or initial value is >= 2^256 (Word() asserts)
+// the 13 operation cells (zk_assign_state_circuit_mpt): the 15 of zk_assign_state_circuit without the root
+enum { SO_RWC, SO_WRITE, SO_TAG, SO_ID, SO_ADDR, SO_FIELD, SO_KLO, SO_KHI, SO_VLO, SO_VHI, SO_ILO, SO_IHI, SO_SEL };
+struct StateMpt {
+  const unsigned char* base;  // the staged operation columns
+  u64 off[13];
+  unsigned char w[13];
+  const unsigned char* flags;  // row flags (bit 0: value is a Word, bit 1: initial value is a Word), may be null
+  u64 n;
+  u64* slots;     // [mask + 1], SM_EMPTY = free
+  u32* key_min;   // [mask + 1] the smallest op index of the key that claimed the slot
+  u32* rank_at;   // [mask + 1] the update rank of that key
+  u64 mask;
+  u32* slot_of;   // [n] the slot of op i's key, ~0: not an MPT op
+  unsigned char* fl;  // [n] bit 0: an MPT op, bit 1: a first touch
+  unsigned long long* stat;  // [0] the first failing op ((i << 2) | SM_FAIL_*, ~0: none), [1] updates, [2] MPT ops
+  const u64 *x_upd, *top_upd, *x_mpt, *top_mpt;  // the two count scans (k_assign_pi_scan)
+  u32* upd_op;  // [U] the op of update u
+  u32* mpt_op;  // [MPT ops] the MPT ops in order
+  u64 n_upd, n_mpt;
+  unsigned char* root;  // the state matrix's root lo column, 8 bytes per row
+  unsigned char* tbase;  // the MPT table's narrow columns
+  u64 toff[12];
+  unsigned char twidth[12];
+};
+ZK_HD Fr sm_cell(const StateMpt& a, int c, u64 i) { return ld_col(a.base + a.off[c], a.w[c], i); }
+ZK_HD bool sm_is(const Fr& v, u64 x) { return v.l[0] == x && !(v.l[1] | v.l[2] | v.l[3]); }
+// the key hash: a multiply-xor over the 16 limbs of the 4 key cells, then a 64-bit finaliser; unkeyed, so the slot
+// of a key is a function of the key and the capacity alone (tests build colliding keys from it)
+ZK_HD u64 state_mpt_hash(const Fr (&k)[4]) {
+  u64 h = 0x243F6A8885A308D3ull;
+#pragma unroll
+  for (int c = 0; c < 4; c++)
+#pragma unroll
+    for (int q = 0; q < 4; q++) h = (h ^ k[c].l[q]) * 0x9E3779B97F4A7C15ull + (u64)(4 * c + q);
+  h ^= h >> 32;
+  h *= 0xD6E8FEB86659FD93ull;
+  h ^= h >> 32;
+  return h;
+}
+// op i's MPT key, false if it is not an Account or Storage op
+ZK_HD bool state_mpt_key(const StateMpt& a, u64 i, Fr (&k)[4]) {
+  const Fr tag = sm_cell(a, SO_TAG, i);
+  if (!sm_is(tag, SM_TAG_STORAGE) && !sm_is(tag, SM_TAG_ACCOUNT)) return false;
+  k[0] = sm_cell(a, SO_ADDR, i);
+  k[1] = sm_cell(a, SO_FIELD, i);
+  k[2] = sm_cell(a, SO_KLO, i);
+  k[3] = sm_cell(a, SO_KHI, i);
+  return true;
+}
+// claim or find the slot of op i's key and lower the key's minimum to i
+ZK_HD void state_mpt_insert(const StateMpt& a, u64 i) {
+  Fr k[4];
+  if (!state_mpt_key(a, i, k)) {
+    a.slot_of[i] = ~0u;
+    a.fl[i] = 0;
+    return;
+  }
+  const u64 h = state_mpt_hash(k), entry = (h & 0xFFFFFFFF00000000ull) | i;
+  u64 b = h & a.mask;
+  for (;;) {
+    const u64 old = atomic_cas_u64(&a.slots[b], SM_EMPTY, entry);
+    if (old == SM_EMPTY) break;
+    if ((old >> 32) == (entry >> 32)) {  // same fingerprint: compare the full key with the claimer's
+      Fr o[4];
+      state_mpt_key(a, (u32)old, o);
+      if (fr_eq(o[0], k[0]) && fr_eq(o[1], k[1]) && fr_eq(o[2], k[2]) && fr_eq(o[3], k[3])) break;
+    }
+    b = (b + 1) & a.mask;
+  }
+  a.slot_of[i] = (u32)b;
+  atomic_min_u32(&a.key_min[b], (u32)i);
+  a.fl[i] = 1;
+}
+// a Word's integer lo + hi 2^128 as 4 limbs; false if it is >= 2^256
+ZK_HD bool sm_word_int(const Fr& lo, const Fr& hi, u64 (&v)[4]) {
+  v[0] = lo.l[0], v[1] = lo.l[1];
+  v[2] = lo.l[2] + hi.l[0];
+  const u64 c2 = v[2] < hi.l[0];
+  const u64 s3 = lo.l[3] + hi.l[1];
+  v[3] = s3 + c2;
+  const bool carry = s3 < hi.l[1] || v[3] < c2;
+  return !(carry || hi.l[2] || hi.l[3]);
+}
+// Word(op.value.int_value()) of a value cell pair: a field value is lo itself, a Word lo + hi 2^128
+ZK_HD bool sm_value(const StateMpt& a, u64 i, int c_lo, bool word, u64 (&v)[4]) {
+  const Fr lo = sm_cell(a, c_lo, i);
+  if (!word) {
+    v[0] = lo.l[0], v[1] = lo.l[1], v[2] = lo.l[2], v[3] = lo.l[3];
+    return true;
+  }
+  return sm_word_int(lo, sm_cell(a, c_lo + 1, i), v);
+}
+ZK_HD unsigned sm_flags(const StateMpt& a, u64 i) { return a.flags ? a.flags[i] : 0; }
+// after every insert: mark op i's first touch, and the reason (SM_FAIL_*) the mirror's loop would stop at it, or 0
+ZK_HD unsigned state_mpt_first(const StateMpt& a, u64 i, unsigned* fail) {
+  *fail = 0;
+  const u32 s = a.slot_of[i];
+  if (s == ~0u) return 0;
+  const bool first = a.key_min[s] == (u32)i;
+  a.fl[i] = first ? 3 : 1;
+  if (first) {
+    const Fr ft = sm_cell(a, SO_FIELD, i);
+    const unsigned f = sm_flags(a, i);
+    u64 v[4];
+    if (sm_is(sm_cell(a, SO_TAG, i), SM_TAG_ACCOUNT) && (ft.l[1] | ft.l[2] | ft.l[3] || ft.l[0] < 1 || ft.l[0] > 4)) *fail = SM_FAIL_FIELD_TAG;
+    else if (!sm_value(a, i, SO_VLO, f & 1, v) || !sm_value(a, i, SO_ILO, f & 2, v)) *fail = SM_FAIL_WORD;
+  }
+  return a.fl[i];
+}
+// the items before j (< n) with a bit of `mask` set, from a count scan
+ZK_HD u64 sm_count_before(const u64* x, const u64* top, const unsigned char* fl, unsigned mask, u64 j) {
+  const u64 c = j / ZK_SEG_CHUNK;
+  u64 v = top[c / PI_SCAN_BLOCK_CHUNKS] + x[c];
+  for (u64 t = c * ZK_SEG_CHUNK; t < j; t++) v += (fl[t] & mask) != 0;
+  return v;
+}
+// op i's place in the ordered MPT-op list and, for a first touch, its update rank
+ZK_HD void state_mpt_compact(const StateMpt& a, u64 i) {
+  const unsigned f = a.fl[i];
+  if (f & 1) a.mpt_op[sm_count_before(a.x_mpt, a.top_mpt, a.fl, 1, i)] = (u32)i;
+  if (f & 2) {
+    const u64 r = sm_count_before(a.x_upd, a.top_upd, a.fl, 2, i);
+    a.upd_op[r] = (u32)i;
+    a.rank_at[a.slot_of[i]] = (u32)r;
+  }
+}
+// row k's root lo: root_prev of the first MPT op after k, or the final root
+ZK_HD void state_mpt_row_root(const StateMpt& a, u64 k) {
+  u64 root = 3 + 5 * a.n_upd;
+  if (k + 1 < a.n) {
+    const u64 j = sm_count_before(a.x_mpt, a.top_mpt, a.fl, 1, k + 1);
+    if (j < a.n_mpt) root = 3 + 5 * (u64)a.rank_at[a.slot_of[a.mpt_op[j]]];
+  }
+  ((u64*)a.root)[k] = root;
+}
+// MPT table row u from the op of update u: address, proof type, key lo, hi, root, 0, root_prev, 0, value lo, hi,
+// value_prev lo, hi, the two values re-split into 128-bit halves
+ZK_HD void state_mpt_table_row(const StateMpt& a, u64 u) {
+  const u64 i = a.upd_op[u];
+  const unsigned f = sm_flags(a, i);
+  const Fr field = sm_cell(a, SO_FIELD, i);
+  const u64 proof = sm_is(sm_cell(a, SO_TAG, i), SM_TAG_STORAGE) ? SM_PROOF_STORAGE_MOD : field.l[0];
+  u64 v[4], p[4];
+  sm_value(a, i, SO_VLO, f & 1, v);
+  sm_value(a, i, SO_ILO, f & 2, p);
+  unsigned char* T = a.tbase;
+  st_width(T + a.toff[0], a.twidth[0], u, sm_cell(a, SO_ADDR, i));
+  T[a.toff[1] + u] = (unsigned char)proof;
+  st_width(T + a.toff[2], a.twidth[2], u, sm_cell(a, SO_KLO, i));
+  st_width(T + a.toff[3], a.twidth[3], u, sm_cell(a, SO_KHI, i));
+  ((u64*)(T + a.toff[4]))[u] = 3 + 5 * (u + 1);
+  T[a.toff[5] + u] = 0;
+  ((u64*)(T + a.toff[6]))[u] = 3 + 5 * u;
+  T[a.toff[7] + u] = 0;
+  st_u128(T + a.toff[8], u, v[0], v[1]);
+  st_u128(T + a.toff[9], u, v[2], v[3]);
+  st_u128(T + a.toff[10], u, p[0], p[1]);
+  st_u128(T + a.toff[11], u, p[2], p[3]);
+}
+
+// host validation of the packed operation columns of zk_assign_state_circuit (15) and zk_assign_state_circuit_mpt (13)
+// (and of the CPU emulation): the row bound, the column format, and the address (column 4) within 160 bits
+static const char* state_ops_error(uint64_t n_rows, int n_cols, const void* packed_ops, uint64_t total_bytes,
+                                   const uint64_t* col_offsets, const uint8_t* col_widths) {
+  if (n_rows >= 0xFFFFFFFFull) return "too many rows (row ids are uint32)";
+  if (!col_offsets || !col_widths) return "the state circuit needs offsets and widths of the operation columns";
+  for (int c = 0; c < n_cols; c++) {
+    const unsigned w = col_widths[c];
+    if (!(w == 0 || w == 1 || w == 2 || w == 4 || w == 8 || w == 16 || w == 32)) return "packed column width must be 0, 1, 2, 4, 8, 16 or 32";
+    if (col_offsets[c] % 32 || col_offsets[c] + (w ? (size_t)w * n_rows : 32) > total_bytes)
+      return "packed column offset misaligned or outside the buffer";
+  }
+  if (col_widths[4] == 32) {  // op.address.to_bytes(20, "little") raises OverflowError beyond 160 bits (state_circuit.py:832)
+    const u64* a = (const u64*)((const unsigned char*)packed_ops + col_offsets[4]);
+    for (u64 r = 0; r < n_rows; r++)
+      if ((a[4 * r + 2] >> 32) || a[4 * r + 3]) return "operation address does not fit 20 bytes (op2row raises OverflowError)";
+  }
+  return nullptr;
+}
+// the hash table of zk_assign_state_circuit_mpt: a power of two >= 2 n slots (at most half full), at least 64
+static u64 state_mpt_slots(u64 n) {
+  u64 cap = 64;
+  while (cap < 2 * n) cap <<= 1;
+  return cap;
 }
 
 #ifdef __CUDACC__
@@ -1157,6 +1368,41 @@ __global__ void __launch_bounds__(256) k_copy_table_write(const __grid_constant_
     pos += total;
     __syncthreads();
   }
+}
+
+// ---- state circuit roots + MPT table (persistent grids, grid stride)
+__global__ void __launch_bounds__(256) k_state_mpt_insert(const __grid_constant__ StateMpt a) {
+  const u64 stride = (u64)gridDim.x * blockDim.x;
+  for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += stride) state_mpt_insert(a, i);
+}
+// first touches, the first failing op (one atomic per failing op: a rejected input), and the two totals with one
+// atomic per warp
+__global__ void __launch_bounds__(256) k_state_mpt_first(const __grid_constant__ StateMpt a) {
+  const u32 lane = threadIdx.x & 31;
+  const u64 stride = (u64)gridDim.x * blockDim.x;
+  for (u64 w = (u64)blockIdx.x * blockDim.x + threadIdx.x - lane; w < a.n; w += stride) {  // warp-uniform
+    const u64 i = w + lane;
+    unsigned f = 0, fail = 0;
+    if (i < a.n) f = state_mpt_first(a, i, &fail);
+    if (fail) atomicMin(a.stat, (unsigned long long)((i << 2) | fail));
+    const u32 upd = __ballot_sync(~0u, f & 2), mpt = __ballot_sync(~0u, f & 1);
+    if (lane == 0) {
+      if (upd) atomicAdd(a.stat + 1, (unsigned long long)__popc(upd));
+      if (mpt) atomicAdd(a.stat + 2, (unsigned long long)__popc(mpt));
+    }
+  }
+}
+__global__ void __launch_bounds__(256) k_state_mpt_compact(const __grid_constant__ StateMpt a) {
+  const u64 stride = (u64)gridDim.x * blockDim.x;
+  for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += stride) state_mpt_compact(a, i);
+}
+__global__ void __launch_bounds__(256) k_state_mpt_rows(const __grid_constant__ StateMpt a) {
+  const u64 stride = (u64)gridDim.x * blockDim.x;
+  for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < a.n; k += stride) state_mpt_row_root(a, k);
+}
+__global__ void __launch_bounds__(256) k_state_mpt_table(const __grid_constant__ StateMpt a) {
+  const u64 stride = (u64)gridDim.x * blockDim.x;
+  for (u64 u = (u64)blockIdx.x * blockDim.x + threadIdx.x; u < a.n_upd; u += stride) state_mpt_table_row(a, u);
 }
 #endif
 

@@ -77,6 +77,7 @@ EXPORTS = [
     "zk_keccak256_batch", "zk_assign_keccak_table", "zk_assign_bytecode_circuit", "zk_assign_state_circuit",
     "zk_assign_copy_circuit", "zk_download_columns", "zk_resident_rows", "zk_assign_exp_circuit", "zk_table_rows",
     "zk_download_table", "zk_assign_pi_circuit", "zk_assign_tx_table", "zk_assign_copy_table", "zk_download_table_flags",
+    "zk_assign_state_circuit_mpt",
 ]
 
 
@@ -114,6 +115,7 @@ def lib() -> ctypes.CDLL:
         L.zk_assign_keccak_table.argtypes = [vp, u64, vp, vp, vp]
         L.zk_assign_bytecode_circuit.argtypes = [vp, u32, u64, vp, vp, vp, vp, vp]
         L.zk_assign_state_circuit.argtypes = [vp, u64, vp, u64, vp, vp, vp, vp]
+        L.zk_assign_state_circuit_mpt.argtypes = [vp, u64, vp, u64, vp, vp, vp, _U64P, vp]
         L.zk_assign_copy_circuit.argtypes = [vp, u64, vp, vp, vp, vp]
         L.zk_download_columns.argtypes = [vp, i32, vp, vp, vp]
         L.zk_resident_rows.argtypes = [vp, i32]
@@ -284,6 +286,28 @@ class Context:
         self._ck(self._L.zk_assign_state_circuit(self._h, pm.n_rows, _host_ptr(pm.buf), pm.nbytes,
                                                  _host_ptr(offs), _host_ptr(widths), None if fl is None else _host_ptr(fl),
                                                  ctypes.c_void_p(stream)), "zk_assign_state_circuit")
+
+    def assign_state_circuit_mpt(self, ops, flags=None, stream: int = 0) -> int:
+        """assign_state_circuit with its mock MPT updates (state_circuit.py:861-933) on the device from the operations
+        alone: `ops` = a PackedMatrix (or canonical uint64[13][n][4]) of the 13 operation cells (the 15 of
+        assign_state_circuit without root lo/hi), `flags` the WordOrValue type bits of value / initial value.  The rows,
+        roots included, REPLACE the resident CIRCUIT_STATE and the updates the resident TABLE_MPT.  Waits for the stream
+        once and returns the number of updates"""
+        from . import packing
+        pm = ops if isinstance(ops, packing.PackedMatrix) else packing.pack_matrix(self._matrix(ops), widths=[32] * 13)
+        assert pm.n_cols == 13
+        self._keep = getattr(self, "_keep", {})
+        self._keep["state_ops"] = pm
+        offs = np.ascontiguousarray(pm.offsets, dtype=np.uint64)
+        widths = np.ascontiguousarray(pm.widths, dtype=np.uint8)
+        fl = None if flags is None else np.ascontiguousarray(flags, dtype=np.uint8)
+        assert fl is None or fl.shape == (pm.n_rows,)
+        n_upd = ctypes.c_uint64(0)
+        self._ck(self._L.zk_assign_state_circuit_mpt(self._h, pm.n_rows, _host_ptr(pm.buf), pm.nbytes, _host_ptr(offs),
+                                                     _host_ptr(widths), None if fl is None else _host_ptr(fl),
+                                                     ctypes.byref(n_upd), ctypes.c_void_p(stream)),
+                 "zk_assign_state_circuit_mpt")
+        return int(n_upd.value)
 
     def assign_copy_circuit(self, events: np.ndarray, data: np.ndarray, is_code_bits=None, stream: int = 0) -> None:
         """CopyCircuit.copy (evm_circuit/typing.py:1010-1147) on the device: `events` uint64[n][16] (include/zkcheck.h), `data`

@@ -198,6 +198,13 @@ def verify_state_circuit(rows: List[Row], tables: Tables, ctx: Optional[native.C
     raise_first_failure(ff, native.CIRCUIT_STATE, "state row")
 
 
+def verify_state_circuit_resident(ctx: native.Context) -> None:
+    """verify_state_circuit over the resident rows and MPT table (assign.assign_state_circuit_mpt leaves both): ONE
+    zk_check(ZK_CIRCUIT_STATE) with wrap-around rotations, raising like verify_state_circuit"""
+    ff, _ = ctx.check(native.CIRCUIT_STATE, 0, ctx.resident_rows(native.CIRCUIT_STATE), 0, native.FLAG_WRAP)
+    raise_first_failure(ff, native.CIRCUIT_STATE, "state row")
+
+
 def check_state_row(row: Row, row_prev: Row, row_next: Row, tables: Tables, ctx: Optional[native.Context] = None) -> None:
     """Reference signature (state_circuit.py:492): checks `row` with its neighbours on the device."""
     ctx = ctx or native.default_context()
